@@ -26,7 +26,6 @@
 // them).  Frames this path does not cover (Left-Right orientation, unaligned pitch, windows wider than 64 samples or taller than
 // 32 rows, more than 1024 windows) are left to k_pf_windows_fast: this kernel sets PfFrame.win2 for the frames it takes.
 #include <cstdio>
-#include <cstdlib>
 
 #include "pf_common.cuh"
 #include "pf_win_common.cuh"
@@ -35,8 +34,7 @@
 namespace epid {
 
 constexpr int WA_WARPS = 8;
-constexpr int WA_SLOT_BIG = 6656;      // bytes per staging slot: 26 rows x 256 B (two 51-sample windows of a 10 mm leaf at 2.56 px/mm), 2 CTAs / SM
-constexpr int WA_SLOT_SMALL = 4416;    // 13 rows x 336 B (three such windows of a 5 mm leaf), 3 CTAs / SM
+constexpr int WA_SLOT = 4416;          // bytes per staging slot: 13 rows x 336 B (three 51-sample windows of a 5 mm leaf at 2.56 px/mm), 3 CTAs / SM
 constexpr int WA_GRID_X = 4;           // CTAs per frame
 constexpr int WA_GMAX = 4;             // pickets per task
 constexpr int WA_KMAX = 4;             // rows per lane in P1: ceil(32 rows / (32 lanes / 4 pickets))
@@ -51,27 +49,57 @@ struct W2Geo {
     int gtot[WA_GMAX + 1];      // median-pool samples of one leaf when pickets are taken g at a time
 };
 
-template <int WA_SLOT, int MINB>
-__global__ void __launch_bounds__(WA_WARPS * 32, MINB)
+// P2 of one band: 2 * median over the nr staged rows (row stride S pixels) of the column pairs t0, t0 + 32, ... < t1, mapped to g
+// units (inv ? k2 - m : m - k2) into out[t].  One call per band: the row count selects the sorting network once, and the loop over
+// the pairs runs inside that instantiation (a call per pair costs a switch, a call and the saves around it for every pair).
+template <int N>
+__device__ __forceinline__ void band_medians_exact(const uint16_t* __restrict__ px, int S, int t0, int t1, uint2* out, int inv, uint32_t k2) {
+    for (int t = t0; t < t1; t += 32) {
+        uint32_t lo, hi;
+        pair_median_exact<N>(px, S, t, lo, hi);
+        out[t] = inv ? make_uint2(k2 - lo, k2 - hi) : make_uint2(lo - k2, hi - k2);
+    }
+}
+static __device__ __noinline__ void band_medians(const uint16_t* __restrict__ px, int S, int nr, int t0, int t1, uint2* out, int inv,
+                                                 uint32_t k2) {
+    switch (nr) {
+#define EPID_MED_CASE(N) case N: band_medians_exact<N>(px, S, t0, t1, out, inv, k2); return;
+        EPID_MED_CASE(6) EPID_MED_CASE(7) EPID_MED_CASE(8) EPID_MED_CASE(9) EPID_MED_CASE(10) EPID_MED_CASE(11)
+        EPID_MED_CASE(12) EPID_MED_CASE(13) EPID_MED_CASE(14) EPID_MED_CASE(15) EPID_MED_CASE(16) EPID_MED_CASE(17)
+        EPID_MED_CASE(18) EPID_MED_CASE(19) EPID_MED_CASE(20) EPID_MED_CASE(21) EPID_MED_CASE(22) EPID_MED_CASE(23)
+        EPID_MED_CASE(24) EPID_MED_CASE(25) EPID_MED_CASE(26) EPID_MED_CASE(27) EPID_MED_CASE(28) EPID_MED_CASE(29)
+        EPID_MED_CASE(30) EPID_MED_CASE(31) EPID_MED_CASE(32)
+#undef EPID_MED_CASE
+        default:
+            for (int t = t0; t < t1; t += 32) {       // fewer than 6 rows (nr <= PF_W2_NRW = 32 in this kernel)
+                uint32_t lo, hi;
+                pair_median_padded<8>(px, S, nr, t, lo, hi);
+                out[t] = inv ? make_uint2(k2 - lo, k2 - hi) : make_uint2(lo - k2, hi - k2);
+            }
+    }
+}
+
+__global__ void __launch_bounds__(WA_WARPS * 32, 3)
 k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ frames, PfFrame* fr, PfWinRec* __restrict__ recs,
                  uint32_t* __restrict__ pools) {
     extern __shared__ __align__(128) unsigned char smraw[];          // WA_WARPS x 2 slots
     __shared__ __align__(8) unsigned long long s_bar[WA_WARPS][2];
     __shared__ W2Geo s_geo;
-    __shared__ int s_a0[PF_P], s_a1[PF_P];
+    __shared__ short s_a0[PF_P], s_a1[PF_P];
     // per group size / group: first band column (view coordinates), vectors per row, first / one-past-last band word that belongs to
     // a window, offset of the band inside the leaf's part of the median pool
-    __shared__ short s_gcs[WA_GMAX + 1][PF_P], s_gnv[WA_GMAX + 1][PF_P], s_gt0[WA_GMAX + 1][PF_P], s_gt1[WA_GMAX + 1][PF_P];
-    __shared__ int s_gofs[WA_GMAX + 1][PF_P];
+    // (row g - 1: groups of g pickets; 16-bit entries: 3.4 KB of static shared memory per CTA, so three resident CTAs leave 8 KB
+    // of an SM's shared memory to kernels of another stream, such as the per-frame re-run of hot-pixel frames)
+    __shared__ short s_gcs[WA_GMAX][PF_P], s_gnv[WA_GMAX][PF_P], s_gt0[WA_GMAX][PF_P], s_gt1[WA_GMAX][PF_P];
+    __shared__ unsigned short s_gofs[WA_GMAX][PF_P];       // < PF_W2_POOL for the group size the frame's leaves use
     __shared__ short s_b0[PF_L], s_nr[PF_L];
     __shared__ unsigned char s_lg[PF_L];                              // pickets per task of this leaf
-    __shared__ int s_toff[PF_L + 1];                                  // tasks before leaf li
+    __shared__ unsigned short s_toff[PF_L + 1];                       // tasks before leaf li (<= PF_W2_WCAP)
     __shared__ int s_moff[PF_L + 1];                                  // median-pool samples before leaf li
     const int fi = blockIdx.y;
     const PfConst& c = *cc;
     PfFrame& f = fr[fi];
     const int tid = threadIdx.x, lane = tid & 31;
-    constexpr bool LDGSTS = false;          // alternative LDGSTS loader; the TMA row copies are the default
     const int wid = __shfl_sync(0xffffffffu, tid >> 5, 0);           // warp-uniform for the compiler
     const int H = c.H, W = c.W;
     const FrameRef frf = frames[fi];
@@ -105,8 +133,8 @@ k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ fr
             const double pidx = (double)f.picket_idx[lane];
             a0 = max((int)(pidx - sp / 2.0), 0);
             a1 = min((int)(pidx + sp / 2.0), W);
-            s_a0[lane] = a0;
-            s_a1[lane] = a1;
+            s_a0[lane] = (short)a0;
+            s_a1[lane] = (short)a1;
             if (a1 - a0 > PF_W2_NCW) bad = 1;
         }
         __syncwarp();
@@ -125,10 +153,10 @@ k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ fr
                 const int ce = hi + ((8 - ((hi + mis) & 7)) & 7);
                 nvec = (ce - cs) >> 3;
                 const int t0 = (lo - cs) >> 1, t1 = empty ? t0 : (hi - cs + 1) >> 1;
-                s_gcs[g][lane] = (short)cs;
-                s_gnv[g][lane] = (short)nvec;
-                s_gt0[g][lane] = (short)t0;
-                s_gt1[g][lane] = (short)t1;
+                s_gcs[g - 1][lane] = (short)cs;
+                s_gnv[g - 1][lane] = (short)nvec;
+                s_gt0[g - 1][lane] = (short)t0;
+                s_gt1[g - 1][lane] = (short)t1;
                 nsamp = 2 * (t1 - t0);
             }
             int inc = nsamp;
@@ -137,7 +165,7 @@ k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ fr
                 const int t = __shfl_up_sync(0xffffffffu, inc, o);
                 if (lane >= o) inc += t;
             }
-            if (lane < ng) s_gofs[g][lane] = inc - nsamp;
+            if (lane < ng) s_gofs[g - 1][lane] = (unsigned short)(inc - nsamp);
             const int nvmax = warp_max(nvec);
             const int tot = __shfl_sync(0xffffffffu, inc, 31);
             if (lane == 0) { s_geo.nvmax[g] = nvmax; s_geo.gtot[g] = tot; }
@@ -167,14 +195,14 @@ k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ fr
                 const int t = __shfl_up_sync(0xffffffffu, inc, o), u = __shfl_up_sync(0xffffffffu, minc, o);
                 if (lane >= o) { inc += t; minc += u; }
             }
-            if (i < ninview) { s_toff[i] = run + inc - cnt; s_moff[i] = mrun + minc - msz; }
+            if (i < ninview) { s_toff[i] = (unsigned short)(run + inc - cnt); s_moff[i] = mrun + minc - msz; }
             run += __shfl_sync(0xffffffffu, inc, 31);
             mrun += __shfl_sync(0xffffffffu, minc, 31);
         }
         if (mrun > PF_W2_POOL) bad = 1;
         bad = __any_sync(0xffffffffu, bad);
         if (lane == 0) {
-            s_toff[ninview] = run;
+            s_toff[ninview] = (unsigned short)run;
             s_moff[ninview] = mrun;
             s_geo.ntasks = run;
             s_geo.ok = bad ? 0 : 1;
@@ -185,7 +213,7 @@ k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ fr
     if (!s_geo.ok) return;
     const int ntasks = s_geo.ntasks;
     const int inv = f.inv;
-    const uint32_t mn = f.mn, mx = f.mx;
+    const uint32_t k2 = inv ? 2u * f.mx : 2u * f.mn;           // 2 * median -> ground / inversion map: inv ? k2 - m : m - k2
     const int sag = c.p.sag_px;
     unsigned char* slot0 = smraw + (size_t)wid * 2 * WA_SLOT;
     const uint32_t bar0 = smem_u32(&s_bar[wid][0]), bar1 = smem_u32(&s_bar[wid][1]);
@@ -196,22 +224,9 @@ k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ fr
     auto issue = [&](int task, int li, int sl) {
         const int G = s_lg[li], g = task - s_toff[li];
         const int b0 = s_b0[li], nr = s_nr[li];
-        const int nvec = s_gnv[G][g], cs = s_gcs[G][g];
+        const int nvec = s_gnv[G - 1][g], cs = s_gcs[G - 1][g];
         if (nr <= 0) return;                         // nothing to copy: the consumer does not wait either
         const int RS = wa_row_stride_bytes(nvec);
-        if (LDGSTS) {
-            const int nv_tot = nr * nvec;
-            const float inv_nvec = 1.0f / (float)nvec;
-            for (int idx = lane; idx < nv_tot; idx += 32) {
-                const int r = (int)(((float)idx + 0.5f) * inv_nvec), v = idx - r * nvec;
-                int row = b0 + r - sag;
-                if (sag) { row %= H; if (row < 0) row += H; }
-                const uint32_t dst = smem_u32(slot0 + (size_t)sl * WA_SLOT + (size_t)r * RS + (size_t)v * 16);
-                const void* src = frf.origin + ((ptrdiff_t)row * frf.pitch + cs + v * 8);
-                asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
-            }
-            return;
-        }
         const uint32_t bar = sl ? bar1 : bar0;
         const uint32_t bytes = (uint32_t)nvec * 16u;
         if (lane == 0) mbar_expect_tx(bar, (uint32_t)nr * bytes);
@@ -228,20 +243,18 @@ k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ fr
     uint32_t ph0 = 0, ph1 = 0;
     int cur = 0, li = 0, li_next = 0;
     if (task < ntasks) { li = leaf_of(task, 0); issue(task, li, 0); }
-    if (LDGSTS) asm volatile("cp.async.commit_group;" ::: "memory");
     for (; task < ntasks; task += tstride, cur ^= 1, li = li_next) {
         if (task + tstride < ntasks) {
             li_next = leaf_of(task + tstride, li);
             issue(task + tstride, li_next, cur ^ 1);     // that slot was released by the __syncwarp at the end of the previous iteration
         }
-        if (LDGSTS) asm volatile("cp.async.commit_group;" ::: "memory");      // (possibly empty) group of the next task
         const int G = s_lg[li], g = task - s_toff[li];
         const int nr = s_nr[li];
-        const int nvec = s_gnv[G][g], cs = s_gcs[G][g];
+        const int nvec = s_gnv[G - 1][g], cs = s_gcs[G - 1][g];
         const int RS = wa_row_stride_bytes(nvec);
         const int Gn = min(G, np - g * G);
-        const int t_lo = s_gt0[G][g], t_hi = s_gt1[G][g];
-        const int boff = s_moff[li] + s_gofs[G][g];                   // the band's first sample in the median pool (even)
+        const int t_lo = s_gt0[G - 1][g], t_hi = s_gt1[G - 1][g];
+        const int boff = s_moff[li] + s_gofs[G - 1][g];                   // the band's first sample in the median pool (even)
         PfWinRec* lrec = frecs + (size_t)li * np + (size_t)g * G;
         if (lane < Gn) {       // header: the shape of the window (empty windows are reported by the analysis kernel) and its samples
             const int a0 = s_a0[g * G + lane], a1 = s_a1[g * G + lane];
@@ -249,8 +262,7 @@ k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ fr
             lrec[lane].moff = (uint32_t)(boff + (a0 - (cs + 2 * t_lo)));
         }
         if (nr <= 0) { __syncwarp(); continue; }
-        if (LDGSTS) { asm volatile("cp.async.wait_group 1;" ::: "memory"); __syncwarp(); }      // everything but the newest group has landed
-        else if (cur) { mbar_wait(bar1, ph1); ph1 ^= 1u; } else { mbar_wait(bar0, ph0); ph0 ^= 1u; }
+        if (cur) { mbar_wait(bar1, ph1); ph1 ^= 1u; } else { mbar_wait(bar0, ph0); ph0 ^= 1u; }
         const unsigned char* band = slot0 + (size_t)cur * WA_SLOT;
         // ---- P1: lanes = (picket of the group, row): rows [k * RPI, (k + 1) * RPI) in pass k
         {
@@ -302,16 +314,7 @@ k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ fr
             }
         }
         // ---- P2: 2 * median over the rows for every pair of band columns between the group's first and last window
-        {
-            const uint16_t* px = reinterpret_cast<const uint16_t*>(band);
-            const int S = RS >> 1;
-            for (int t = t_lo + lane; t < t_hi; t += 32) {
-                const uint2 mm = pair_median_any(px, S, nr, t);
-                const uint32_t g0 = inv ? 2u * mx - mm.x : mm.x - 2u * mn;
-                const uint32_t g1 = inv ? 2u * mx - mm.y : mm.y - 2u * mn;
-                *reinterpret_cast<uint2*>(pool + boff + 2 * (t - t_lo)) = make_uint2(g0, g1);
-            }
-        }
+        band_medians(reinterpret_cast<const uint16_t*>(band), RS >> 1, nr, t_lo + lane, t_hi, reinterpret_cast<uint2*>(pool + boff) - t_lo, inv, k2);
         __syncwarp();       // every lane is done with the slot: the next iteration may overwrite the other one... and this one after it
     }
 }
@@ -436,19 +439,9 @@ size_t pf_win2_scratch_bytes(int n) {
 int launch_pf_windows2(epid_ctx* ctx, cudaStream_t stream, const PfConst* cst, const FrameRef* refs, PfFrame* fr, PfWinRec* recs, PfWin* wins,
                        int n, PfTimers* tm) {
     uint32_t* pools = reinterpret_cast<uint32_t*>(reinterpret_cast<char*>(recs) + ((sizeof(PfWinRec) * (size_t)n * PF_W2_WCAP + 255) / 256) * 256);
-    static int gx = 0;
-    if (gx == 0) { const char* e = getenv("EPID_WA_GRID"); gx = e ? atoi(e) : WA_GRID_X; if (gx < 1 || gx > 64) gx = WA_GRID_X; }
-    static int small_slots = -1;
-    if (small_slots < 0) { const char* e = getenv("EPID_WA_SMALL"); small_slots = e ? atoi(e) : 1; }
-    if (small_slots == 1) {
-        const size_t smem = (size_t)WA_WARPS * 2 * WA_SLOT_SMALL;
-        EPID_SMEM_OPT_IN(ctx, (k_pf_win_medians<WA_SLOT_SMALL, 3>), smem);
-        k_pf_win_medians<WA_SLOT_SMALL, 3><<<dim3(gx, n), WA_WARPS * 32, smem, stream>>>(cst, refs, fr, recs, pools);
-    } else {
-        const size_t smem = (size_t)WA_WARPS * 2 * WA_SLOT_BIG;
-        EPID_SMEM_OPT_IN(ctx, (k_pf_win_medians<WA_SLOT_BIG, 2>), smem);
-        k_pf_win_medians<WA_SLOT_BIG, 2><<<dim3(gx, n), WA_WARPS * 32, smem, stream>>>(cst, refs, fr, recs, pools);
-    }
+    const size_t smem = (size_t)WA_WARPS * 2 * WA_SLOT;
+    EPID_SMEM_OPT_IN(ctx, k_pf_win_medians, smem);
+    k_pf_win_medians<<<dim3(WA_GRID_X, n), WA_WARPS * 32, smem, stream>>>(cst, refs, fr, recs, pools);
     ctx->launches++;
     if (tm) { int rc = tm->mark(stream, PF_STAGE_WIN_MEDIANS); if (rc != EPID_OK) return rc; }
     k_pf_win_fwxm<<<dim3(PF_W2_WCAP / WB_THREADS, n), WB_THREADS, 0, stream>>>(cst, fr, recs, pools, wins);

@@ -6,7 +6,6 @@ cat gpurun_out/r2a_pytest_pf.log
 {
 python tools/r2_stages.py --win2 0
 python tools/r2_stages.py --win2 1
-for g in 2 3 6 8; do EPID_WA_GRID=$g python tools/r2_stages.py --win2 1; done
 python tools/r2_stages.py --win2 1 --mixed 5
 python tools/r2_stages.py --win2 1 --frames 64
 } 2>&1 | tee gpurun_out/r2a_stages.log

@@ -6,8 +6,6 @@ cat gpurun_out/r2b_pytest_pf.log
 {
 python tools/r2_stages.py --win2 0
 python tools/r2_stages.py --win2 1
-EPID_WA_LOADER=1 python tools/r2_stages.py --win2 1
-EPID_WA_GRID=2 python tools/r2_stages.py --win2 1
 python tools/r2_stages.py --win2 1 --mixed 5
 } 2>&1 | tee gpurun_out/r2b_stages.log
 timeout 300 ncu --set full --clock-control none --import-source on -k regex:k_pf_win_medians -s 1 -c 1 -o gpurun_out/prof_wmed_r2b -f python tools/prof_pf.py 1 512 > gpurun_out/r2b_ncu1.log 2>&1

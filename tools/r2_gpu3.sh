@@ -4,9 +4,6 @@ python -m pytest tests/test_gpu_pf.py tests/test_gpu_metrics.py tests/test_gpu_w
 cat gpurun_out/r2c_pytest_pf.log
 {
 python tools/r2_stages.py --win2 1
-EPID_WA_LOADER=1 python tools/r2_stages.py --win2 1
-EPID_WA_GRID=2 python tools/r2_stages.py --win2 1
-EPID_WA_GRID=6 python tools/r2_stages.py --win2 1
 python tools/r2_stages.py --win2 1 --frames 64
 } 2>&1 | tee gpurun_out/r2c_stages.log
 timeout 300 ncu --set full --clock-control none --import-source on -k regex:k_pf_win_medians -s 1 -c 1 -o gpurun_out/prof_wmed_r2c -f python tools/prof_pf.py 1 512 > gpurun_out/r2c_ncu1.log 2>&1

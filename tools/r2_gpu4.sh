@@ -3,7 +3,6 @@ mkdir -p gpurun_out
 python -m pytest tests/test_gpu_pf.py -x -q -m gpu 2>&1 | tail -5 | tee gpurun_out/r2d_pytest_pf.log
 {
 python tools/r2_stages.py --win2 1
-EPID_WA_LOADER=1 python tools/r2_stages.py --win2 1
 python tools/r2_stages.py --win2 1 --mixed 5
 } 2>&1 | tee gpurun_out/r2d_stages.log
 timeout 300 ncu --set full --clock-control none --import-source on -k regex:k_pf_win_medians -s 1 -c 1 -o gpurun_out/prof_wmed_r2d -f python tools/prof_pf.py 1 512 > gpurun_out/r2d_ncu1.log 2>&1
