@@ -63,6 +63,20 @@ def has_noise(a) -> bool:
     return bool(max_is_extreme or min_is_extreme)
 
 
+def orientation_ranges(img):
+    """pf:1501-1526 on the ground + normalised image: (orientation, row range, column range).  The orientation is LEFT_RIGHT
+    when the p99 - p85 range of the per-column sums is below that of the per-row sums."""
+    temp = img.copy()
+    med = np.median(temp)
+    temp[temp < med] = med
+    row_sum = np.sum(temp, 0)
+    col_sum = np.sum(temp, 1)
+    row80, row90 = np.percentile(row_sum, [85, 99])
+    col80, col90 = np.percentile(col_sum, [85, 99])
+    row_range, col_range = row90 - row80, col90 - col80
+    return (LEFT_RIGHT if row_range < col_range else UP_DOWN), row_range, col_range
+
+
 def corner_inversion_needed(a, box_size=10, position=(0.01, 0.01)) -> bool:
     """img:881-897"""
     row_pos = max(int(position[0] * a.shape[0]), 1)
@@ -150,15 +164,8 @@ def pf_analyze(frame, dpmm, *, crop_mm=3, filter=None, mlc="Millennium", toleran
     H, W = img.shape
     out["shape"] = (H, W)
 
-    def _orientation():  # pf:1501-1526
-        temp = img.copy()
-        med = np.median(temp)
-        temp[temp < med] = med
-        row_sum = np.sum(temp, 0)
-        col_sum = np.sum(temp, 1)
-        row80, row90 = np.percentile(row_sum, [85, 99])
-        col80, col90 = np.percentile(col_sum, [85, 99])
-        return LEFT_RIGHT if (row90 - row80) < (col90 - col80) else UP_DOWN
+    def _orientation():
+        return orientation_ranges(img)[0]
 
     if orientation is None:
         orient = None

@@ -972,22 +972,6 @@ using namespace epid;
 
 namespace {
 
-PctPlan field_pct_plan(int n, double q_percent) {   // numpy 'linear' virtual index
-    const double q = q_percent / 100.0;
-    const double vi = (double)n * q + (1.0 + q * (1.0 - 1.0 - 1.0)) - 1.0;
-    double prev = floor(vi);
-    PctPlan p;
-    p.gamma = vi - prev;
-    double next = prev + 1.0;
-    if (prev < 0) prev = 0;
-    if (next < 0) next = 0;
-    if (prev > n - 1) prev = n - 1;
-    if (next > n - 1) next = n - 1;
-    p.prev = (int)prev;
-    p.next = (int)next;
-    return p;
-}
-
 __global__ void k_field_refs(const uint16_t* base, int n, int H, int W, FrameRef* refs) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -1019,9 +1003,9 @@ extern "C" int32_t epid_field_analyze(epid_ctx* ctx, const epid_batch* frames, c
     hc.p = *p;
     hc.H = H;
     hc.W = W;
-    hc.p5 = field_pct_plan(H * W, 5.0);
-    hc.p50 = field_pct_plan(H * W, 50.0);
-    hc.p95 = field_pct_plan(H * W, 95.0);
+    hc.p5 = pct_plan(H * W, 5.0);
+    hc.p50 = pct_plan(H * W, 50.0);
+    hc.p95 = pct_plan(H * W, 95.0);
     hc.n_expect[0] = epid_field_profile_len(W, p->dpmm, p->interpolation, p->interpolation_resolution_mm);
     hc.n_expect[1] = epid_field_profile_len(H, p->dpmm, p->interpolation, p->interpolation_resolution_mm);
     int nmax = 10 * (H > W ? H : W);

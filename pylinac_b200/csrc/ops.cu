@@ -341,6 +341,9 @@ int32_t epid_frame_stats(epid_ctx* ctx, const epid_batch* b, int32_t r0, int32_t
                          int32_t nq, double* mn, double* mx, double* sum, double* rowsum, double* colsum, double* pct) {
     EPID_REQUIRE(ctx && b, EPID_ERR_INVALID, "NULL argument");
     EPID_REQUIRE(nq >= 0 && 2 * nq <= STATS_MAX_RANKS, EPID_ERR_UNSUPPORTED, "at most %d percentiles per call", STATS_MAX_RANKS / 2);
+    EPID_REQUIRE(nq == 0 || q_percent, EPID_ERR_INVALID, "NULL percentiles");
+    for (int k = 0; k < nq; k++)   // NaN fails both comparisons
+        EPID_REQUIRE(q_percent[k] >= 0.0 && q_percent[k] <= 100.0, EPID_ERR_INVALID, "Percentiles must be in the range [0, 100]");
     EPID_CUDA(cudaSetDevice(ctx->device));
     const uint16_t* base;
     uint16_t* tmp;
@@ -353,17 +356,10 @@ int32_t epid_frame_stats(epid_ctx* ctx, const epid_batch* b, int32_t r0, int32_t
     const int npix = vh * vw;
     std::vector<double> gam(nq);
     for (int k = 0; k < nq; k++) {
-        const double q = q_percent[k] / 100.0;
-        EPID_REQUIRE(q >= 0.0 && q <= 1.0, EPID_ERR_INVALID, "Percentiles must be in the range [0, 100]");
-        const double vi = (double)npix * q + (1.0 + q * (1.0 - 1.0 - 1.0)) - 1.0;
-        double prev = floor(vi), next = prev + 1.0;
-        gam[k] = vi - prev;
-        if (prev < 0) prev = 0;
-        if (next < 0) next = 0;
-        if (prev > npix - 1) prev = npix - 1;
-        if (next > npix - 1) next = npix - 1;
-        g.ranks[2 * k] = (uint32_t)prev;
-        g.ranks[2 * k + 1] = (uint32_t)next;
+        const PctPlan pp = pct_plan(npix, q_percent[k]);
+        gam[k] = pp.gamma;
+        g.ranks[2 * k] = (uint32_t)pp.prev;
+        g.ranks[2 * k + 1] = (uint32_t)pp.next;
     }
     g.nranks = 2 * nq;
     g.box = 0;

@@ -399,23 +399,6 @@ k_pf_windows(const PfConst* __restrict__ cc, const FrameRef* __restrict__ frames
 }
 
 // ------------------------------------------------------------------------------------------------ host side
-static PctPlan pct_plan(int n, double q_percent) {
-    // numpy 'linear' (numpy/lib/_function_base_impl.py: _compute_virtual_index, _get_indexes, _get_gamma)
-    const double q = q_percent / 100.0;
-    const double vi = (double)n * q + (1.0 + q * (1.0 - 1.0 - 1.0)) - 1.0;
-    double prev = floor(vi);
-    double next = prev + 1.0;
-    PctPlan p;
-    p.gamma = vi - prev;
-    if (prev < 0) prev = 0;
-    if (next < 0) next = 0;
-    if (prev > n - 1) prev = n - 1;
-    if (next > n - 1) next = n - 1;
-    p.prev = (int)prev;
-    p.next = (int)next;
-    return p;
-}
-
 struct PfWork {   // carved out of ctx->scratch
     FrameRef* refs;
     FrameRef* refs_b;        // ping-pong destination refs for median passes

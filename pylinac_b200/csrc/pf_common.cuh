@@ -19,8 +19,6 @@ constexpr int WIN_MAX_NC = 1024;          // samples along leaf travel
 constexpr int WIN_MAX_NR = 64;            // samples across the leaf
 constexpr int FIN_THREADS = 256;
 
-struct PctPlan { int prev, next; double gamma; };
-
 // internal status of a frame whose decisions the single-pass front end could not certify (or that _check_for_noise may flag): the
 // fast pipeline skips it and the caller re-runs exactly that frame through the exact-histogram pipeline (never visible to callers)
 constexpr int PF_STATUS_DEFERRED = 90;

@@ -654,22 +654,6 @@ using namespace epid;
 
 namespace {
 
-PctPlan star_pct_plan(int n, double q_percent) {   // numpy 'linear' virtual index (same arithmetic as pf.cu pct_plan)
-    const double q = q_percent / 100.0;
-    const double vi = (double)n * q + (1.0 + q * (1.0 - 1.0 - 1.0)) - 1.0;
-    double prev = floor(vi);
-    PctPlan p;
-    p.gamma = vi - prev;
-    double next = prev + 1.0;
-    if (prev < 0) prev = 0;
-    if (next < 0) next = 0;
-    if (prev > n - 1) prev = n - 1;
-    if (next > n - 1) next = n - 1;
-    p.prev = (int)prev;
-    p.next = (int)next;
-    return p;
-}
-
 __global__ void k_star_refs(const uint16_t* base, int n, int H, int W, int top, int left, FrameRef* full, FrameRef* central) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
@@ -703,10 +687,10 @@ extern "C" int32_t epid_starshot_analyze(epid_ctx* ctx, const epid_batch* frames
     hc.left = (int)((double)W / 3);
     hc.ch = hc.top * 2 - hc.top;
     hc.cw = hc.left * 2 - hc.left;
-    hc.p4 = star_pct_plan(H * W, 4.0);
-    hc.p50 = star_pct_plan(H * W, 50.0);
-    hc.p96 = star_pct_plan(H * W, 96.0);
-    hc.p90 = star_pct_plan(hc.ch * hc.cw, 90.0);
+    hc.p4 = pct_plan(H * W, 4.0);
+    hc.p50 = pct_plan(H * W, 50.0);
+    hc.p96 = pct_plan(H * W, 96.0);
+    hc.p90 = pct_plan(hc.ch * hc.cw, 90.0);
     hc.nmax = 10 * (H > W ? H : W) + 64;
     hc.max_sigma = max_sigma;
     hc.npad = hc.nmax + 2 * (int)(4.0 * max_sigma + 0.5) + 8;

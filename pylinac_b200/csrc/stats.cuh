@@ -1,5 +1,7 @@
 // Frame-statistics kernel interface (internal).
 #pragma once
+#include <cmath>
+
 #include "common.cuh"
 
 namespace epid {
@@ -35,6 +37,29 @@ struct FrameStats {  // per frame, device memory
     unsigned long long corner_sum;  // sum over the four corner boxes
     uint32_t ostat[STATS_MAX_RANKS];
 };
+
+// np.percentile(a, q_percent) with method="linear" over n values reads the sorted values at ranks prev and next and interpolates with
+// gamma.  numpy's virtual index for "linear" is (n - 1) * q with q = q_percent / 100; written any other way it rounds differently for
+// some (n, q) and the percentile moves by many ulps.  An index at or past n - 1 takes the last value, one below 0 the first.
+struct PctPlan { int prev, next; double gamma; };
+
+__host__ __device__ inline PctPlan pct_plan(int n, double q_percent) {
+    const double vi = (double)(n - 1) * (q_percent / 100.0);
+    PctPlan p;
+    if (vi >= (double)(n - 1)) {
+        p.prev = p.next = n - 1;
+        p.gamma = 0.0;
+    } else if (vi < 0.0) {
+        p.prev = p.next = 0;
+        p.gamma = 0.0;
+    } else {
+        const double prev = floor(vi);
+        p.prev = (int)prev;
+        p.next = p.prev + 1;
+        p.gamma = vi - prev;
+    }
+    return p;
+}
 
 int make_stats_geom(StatsGeom* g, int H, int W);
 

@@ -65,21 +65,6 @@ struct WlFrame {
 
 __device__ __forceinline__ uint32_t wl_T(const WlFrame& f, uint32_t v) { return f.flip ? f.S - v : v; }
 
-// numpy 'linear' percentile plan (np.percentile -> _compute_virtual_index, _get_gamma)
-__device__ __forceinline__ void wl_pct_plan(uint32_t n, double q_percent, uint32_t* prev, uint32_t* next, double* gamma) {
-    const double q = q_percent / 100.0;
-    const double vi = (double)n * q + (1.0 + q * (1.0 - 1.0 - 1.0)) - 1.0;
-    double pv = floor(vi);
-    *gamma = vi - pv;
-    double nx = pv + 1.0;
-    if (pv < 0) pv = 0;
-    if (nx < 0) nx = 0;
-    if (pv > (double)n - 1) pv = (double)n - 1;
-    if (nx > (double)n - 1) nx = (double)n - 1;
-    *prev = (uint32_t)pv;
-    *next = (uint32_t)nx;
-}
-
 // ------------------------------------------------------------------------------------------------ histogram
 constexpr int WL_HSLOTS = 4096;        // direct-mapped shared-memory cache of histogram bins (slot = value mod 4096)
 constexpr int WL_HPARTS = 8;           // CTAs per frame
@@ -191,8 +176,11 @@ k_wl_front(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, ui
     uint32_t n = (uint32_t)H * (uint32_t)W;
     if (tid == 0) {
         const double qs[3] = {0.01, 50.0, 99.99};
-        double g_;
-        for (int k = 0; k < 3; k++) wl_pct_plan(n, qs[k], &s.ranks[2 * k], &s.ranks[2 * k + 1], &g_);
+        for (int k = 0; k < 3; k++) {
+            const PctPlan pp = pct_plan((int)n, qs[k]);
+            s.ranks[2 * k] = pp.prev;
+            s.ranks[2 * k + 1] = pp.next;
+        }
     }
     __syncthreads();
     wl_hist_query(hist, &s, 6);
@@ -201,12 +189,7 @@ k_wl_front(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, ui
     {
         const double qs[3] = {0.01, 50.0, 99.99};
         double p[3];
-        for (int k = 0; k < 3; k++) {
-            uint32_t a, b;
-            double g;
-            wl_pct_plan(n, qs[k], &a, &b, &g);
-            p[k] = np_lerp((double)s.values[2 * k], (double)s.values[2 * k + 1], g);
-        }
+        for (int k = 0; k < 3; k++) p[k] = np_lerp((double)s.values[2 * k], (double)s.values[2 * k + 1], pct_plan((int)n, qs[k]).gamma);
         flip = fabs(p[1] - p[0]) > fabs(p[1] - p[2]) ? 1 : 0;
         S = s.first + s.last;                      // invert(): -a + max + min of the uncropped frame
     }
@@ -222,10 +205,9 @@ k_wl_front(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, ui
         const int h = H - 2 * crop, w = W - 2 * crop;
         if (h <= 4 || w <= 4) break;
         n = (uint32_t)h * (uint32_t)w;
-        uint32_t r5a, r5b, r9a, r9b;
-        double g5, g9;
-        wl_pct_plan(n, 5.0, &r5a, &r5b, &g5);
-        wl_pct_plan(n, 99.5, &r9a, &r9b, &g9);
+        const PctPlan p5 = pct_plan((int)n, 5.0), p9 = pct_plan((int)n, 99.5);
+        const uint32_t r5a = p5.prev, r5b = p5.next, r9a = p9.prev, r9b = p9.next;
+        const double g5 = p5.gamma, g9 = p9.gamma;
         if (tid == 0) {
             // T-domain rank k = raw rank n - 1 - k when flipped (T is decreasing)
             s.ranks[0] = flip ? n - 1 - r5a : r5a; s.ranks[1] = flip ? n - 1 - r5b : r5b;
@@ -279,10 +261,9 @@ k_wl_front(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, ui
     // ---- ground() / normalize() constants and the field threshold (winston_lutz.py:711-712, 764-780)
     const int h = H - 2 * crop, w = W - 2 * crop;
     n = (uint32_t)h * (uint32_t)w;
-    uint32_t r5a, r5b, r9a, r9b;
-    double g5, g9;
-    wl_pct_plan(n, 5.0, &r5a, &r5b, &g5);
-    wl_pct_plan(n, 99.9, &r9a, &r9b, &g9);
+    const PctPlan p5 = pct_plan((int)n, 5.0), p9 = pct_plan((int)n, 99.9);
+    const uint32_t r5a = p5.prev, r5b = p5.next, r9a = p9.prev, r9b = p9.next;
+    const double g5 = p5.gamma, g9 = p9.gamma;
     if (tid == 0) {
         s.ranks[0] = flip ? n - 1 - r5a : r5a; s.ranks[1] = flip ? n - 1 - r5b : r5b;
         s.ranks[2] = flip ? n - 1 - r9a : r9a; s.ranks[3] = flip ? n - 1 - r9b : r9b;
