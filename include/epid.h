@@ -615,6 +615,24 @@ int32_t epid_hough_candidates(epid_ctx* ctx, const epid_batch* accum, int32_t mi
                               int32_t cap, int32_t* cand_yxv, int32_t* count, int32_t* global_max, epid_batch** filtered);
 int32_t epid_gather_i32(epid_ctx* ctx, const epid_batch* img, int32_t npts, const int32_t* yx, int32_t* values);
 
+/* ----------------------------------------------------------------------------------------- Varian XIM pixel decode
+ * XIM._parse_lookup_table / _parse_compressed_bytes / _get_diffs (core/image.py:1186-1309) for a batch of n files that share
+ * h x w and bytes_per_pixel.  arena: host memory (page-locked for a DMA copy; 16-byte aligned) holding every file's lookup table
+ * and compressed pixel buffer; desc[f] = {lookup offset, lookup bytes, pixel offset, pixel bytes} (int64 [n][4], offsets 16-byte
+ * aligned, inside the arena).  One H2D copy of the arena and one launch sequence for the whole batch.
+ * dtype: the reference's dtype (EPID_I16 for bpp 1 and 2 -- bpp 1 values are int8, sign-extended --, EPID_I32 for bpp 4,
+ * EPID_I64 for bpp 8), or EPID_U16: the reference's values checked against [0, 65535] (EPID_XIM_U16_RANGE, never wrapped).
+ * status[f] (host, int32 [n]): EPID_XIM_*.  The frames of a failed status hold unspecified values.  h >= 2 (the reference raises
+ * ValueError for one row); bpp outside {1, 2, 4, 8} returns EPID_ERR_INVALID (ValueError, like the reference). */
+enum {
+    EPID_XIM_OK = 0,
+    EPID_XIM_LOOKUP_CODE3 = 1,     /* a 2-bit code 3 anywhere in the lookup table: KeyError (LOOKUP_CONVERSION[3]) */
+    EPID_XIM_SHORT_BUFFER = 2,     /* the pixel buffer holds fewer bytes than the raw head + the coded diffs: ValueError */
+    EPID_XIM_U16_RANGE = 3         /* EPID_U16 output: a value outside [0, 65535]: ValueError (like image.frame_u16) */
+};
+int32_t epid_xim_decode(epid_ctx* ctx, const void* arena, size_t arena_bytes, const int64_t* desc, int32_t n, int32_t h, int32_t w,
+                        int32_t bpp, int32_t dtype, int32_t* status, epid_batch** out);
+
 /* ----------------------------------------------------------------------------------------- multi-GPU (NCCL)
  * The batch shards by frame index with no data-path collective; the only exchange is the final gather of the
  * fixed-size per-frame result structs (SURVEY.md 8e).  id: 128-byte ncclUniqueId created by rank 0. */

@@ -333,6 +333,7 @@ _SIGNATURES = {
     "epid_comm_info": [_P, C.POINTER(C.c_int32), C.POINTER(C.c_int32)],
     "epid_gather_results": [_P, _P, C.c_size_t, _P],
     "epid_barrier": [_P],
+    "epid_xim_decode": [_P, _P, C.c_size_t, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, C.POINTER(_P)],
 }
 
 
@@ -559,6 +560,22 @@ class _PinnedPool:
 
 
 _RESULT_POOL = _PinnedPool()
+
+
+XIM_OK, XIM_LOOKUP_CODE3, XIM_SHORT_BUFFER, XIM_U16_RANGE = 0, 1, 2, 3
+
+
+def xim_decode(ctx: Context, arena: np.ndarray, desc: np.ndarray, h: int, w: int, bpp: int, dtype) -> tuple[Batch, np.ndarray]:
+    """epid_xim_decode: arena (uint8, 16-byte aligned) + desc int64 [n, 4] -> (device Batch [n, h, w], int32 status [n])"""
+    a = np.ascontiguousarray(arena, dtype=np.uint8)
+    d = np.ascontiguousarray(desc, dtype=np.int64).reshape(-1, 4)
+    if a.ctypes.data % 16:
+        raise ValueError("the XIM arena must be 16-byte aligned")
+    status = np.zeros(len(d), np.int32)
+    h_out = _P()
+    check(lib().epid_xim_decode(ctx.handle, _ptr(a), a.nbytes, _ptr(d), len(d), int(h), int(w), int(bpp), _NP2DT[np.dtype(dtype)],
+                                _ptr(status), C.byref(h_out)))
+    return Batch(ctx, h_out), status
 
 
 def frame_stats(ctx: Context, batch: Batch, view=None, percentiles=()):

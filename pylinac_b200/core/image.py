@@ -653,3 +653,36 @@ class LinacDicomImage(DicomImage):
     @property
     def couch_angle(self) -> float:
         return self._axis("couch", "PatientSupportAngle")
+
+
+class XIM(BaseImage):
+    """core/image.py:1105-1318: a Varian .xim image (TrueBeam / Halcyon EPID and kV, IsoCal and MPC exports).  The header and
+    property walk is the reference's (pylinac_b200.xim); the compressed pixels are decoded on the GPU (csrc/xim.cu) through the
+    same entry point as batched ingest, with n = 1.  Export (save_as / as_dicom) is not provided."""
+
+    array: np.ndarray
+    properties: dict
+
+    def __init__(self, file_path: str | Path, read_pixels: bool = True):
+        from .. import xim
+
+        super().__init__(path=file_path)
+        hd = xim.walk(self.path, read_pixels=read_pixels)
+        if hd.compression and read_pixels:
+            self.array = xim.decode_file(hd)
+            if hd.trailer_error is not None:
+                raise hd.trailer_error
+        for name in ("format_id", "format_version", "img_width_px", "img_height_px", "bits_per_pixel", "bytes_per_pixel",
+                     "compression", "num_hist_bins", "histogram", "num_properties", "properties"):
+            setattr(self, name, getattr(hd, name))
+        if hd.compression:
+            self.lookup_table = hd.lookup_table
+        else:
+            self.pixel_buffer = hd.pixel_buffer
+
+    @property
+    def dpmm(self) -> float:  # core/image.py:1311-1318
+        """The dots/mm value of the XIM images. The value appears to be in cm in the file."""
+        if self.properties["PixelWidth"] != self.properties["PixelHeight"]:
+            raise ValueError("The XIM image does not have the same pixel height and width")
+        return 1 / (10 * self.properties["PixelHeight"])
