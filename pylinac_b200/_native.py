@@ -24,11 +24,7 @@ _NP2DT = {np.dtype(np.uint8): U8, np.dtype(np.uint16): U16, np.dtype(np.int32): 
 _DT2NP = {v: k for k, v in _NP2DT.items()}
 
 OPT_PF_EXACT_ONLY = 1
-OPT_PF_LEAFBAND = 2
 OPT_PF_WIN2 = 3
-OPT_PF_SPLIT = 4
-OPT_PF_FAST_REDO = 5
-OPT_PF_OVERLAP_REDO = 6
 OPT_STATS_EXACT = 7
 CTR_PF_FALLBACKS = 1
 CTR_PF_REDONE_FRAMES = 2
@@ -650,7 +646,7 @@ def pf_bench(ctx: Context, batch: Batch, params: PFParams, iters: int):
 
 
 PF_STAGE_NAMES = ("k_pf_init + k_pf_pilot", "k_pf_stream", "k_pf_tail", "k_pf_windows_fast", "k_pf_windows (generic)", "k_pf_finalize",
-                  "exact front end (fallback)", "k_pf_leafband", "k_pf_win_medians", "k_pf_win_fwxm")
+                  "exact front end (fallback)", "k_pf_win_medians", "k_pf_win_fwxm")
 
 
 def pf_bench_timed(ctx: Context, batch: Batch, params: PFParams, iters: int):

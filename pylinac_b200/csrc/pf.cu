@@ -599,8 +599,7 @@ static int pf_run(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, 
     hc.W = W;
     hc.meas_cap = meas_cap;
     hc.post_filter = 0;
-    hc.leafband = ctx->pf_leafband ? 1 : 0;
-    hc.win2 = (ctx->pf_win2 && !hc.leafband) ? 1 : 0;
+    hc.win2 = ctx->pf_win2 ? 1 : 0;
     const int npix = H * W;
     hc.lo = pct_plan(npix, 0.5);
     hc.hi = pct_plan(npix, 99.5);
@@ -726,11 +725,6 @@ static int pf_run(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, 
     }   // !fast
     {
         // fast path for ordinary window sizes, then the generic kernel for whatever it left marked (valid == -1)
-        if (hc.leafband) {
-            rc = launch_pf_leafband(ctx, stream, w.cst, w.refs, w.fr, w.wins, n);
-            if (rc != EPID_OK) return rc;
-            if (tm) { rc = tm->mark(stream, PF_STAGE_LEAFBAND); if (rc != EPID_OK) return rc; }
-        }
         if (hc.win2) {
             rc = launch_pf_windows2(ctx, stream, w.cst, w.refs, w.fr, w.winrec, w.wins, n, tm);
             if (rc != EPID_OK) return rc;
@@ -750,8 +744,7 @@ static int pf_run(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, 
     return EPID_OK;
 }
 
-// Per-frame fallback: the m frames the fast pipeline deferred (w.sel_idx, ascending) are re-run by the exact-histogram pipeline in
-// sub-batches whose work area lives in ctx->scratch2, and their result rows are scattered into the batch's device result arrays.
+// work area of the per-frame re-run of deferred frames (pf_redo_deferred)
 static int ensure_scratch2(epid_ctx* ctx, size_t bytes) {
     if (ctx->scratch2_bytes >= bytes) return EPID_OK;
     if (ctx->scratch2) { EPID_CUDA(cudaStreamSynchronize(ctx->stream)); EPID_CUDA(cudaFree(ctx->scratch2)); ctx->scratch2 = nullptr; ctx->scratch2_bytes = 0; }
@@ -769,18 +762,17 @@ static bool pf_fast_ok(const epid_ctx* ctx, const epid_pf_params* p, int H0, int
 
 // Re-run of the m frames the fast pass deferred (w.sel_idx, ascending) on `stream`, in sub-batches whose work area lives in
 // ctx->scratch2; result rows are scattered into the batch's device result arrays (after `after`, the event that marks the end of the
-// batch's own pass, when the re-run is overlapped with it on another stream).  ctx->pf_fast_redo: first the certified-noise fast
-// re-run (pf_run with PfRedoIn), then the exact-histogram pipeline for whatever that deferred again; otherwise exact for all.
+// batch's own pass, when the re-run is overlapped with it on another stream).  First the certified-noise fast re-run (pf_run with
+// PfRedoIn), then the exact-histogram pipeline for whatever that deferred again.  Only called when the batch took the fast pipeline.
 static int pf_redo_deferred(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, int m, int H0, int W0, const epid_pf_params* p,
                             int meas_cap, PfWork& w, uint16_t** pools, cudaEvent_t after = nullptr) {
     const int H = H0 - 2 * p->crop_px, W = W0 - 2 * p->crop_px;
     const int Wp = (W + 7) / 8 * 8;
     const int chunk = m < PF_REDO_CHUNK ? m : PF_REDO_CHUNK;
-    const bool fast_redo = ctx->pf_fast_redo && pf_fast_ok(ctx, p, H0, W0);
     PfWork rw;
     carve(rw, nullptr, chunk, H, W, meas_cap);
     const size_t work_bytes = align_up(rw.total, 256);
-    const size_t pool_bytes = fast_redo ? align_up(sizeof(uint16_t) * (size_t)chunk * H * Wp + 512, 256) : 0;
+    const size_t pool_bytes = align_up(sizeof(uint16_t) * (size_t)chunk * H * Wp + 512, 256);
     int rc = ensure_scratch2(ctx, work_bytes + pool_bytes);
     if (rc != EPID_OK) return rc;
     carve(rw, (char*)ctx->scratch2, chunk, H, W, meas_cap);
@@ -790,19 +782,12 @@ static int pf_redo_deferred(epid_ctx* ctx, cudaStream_t stream, const uint16_t* 
     bool waited = after == nullptr;
     for (int c0 = 0; c0 < m; c0 += chunk) {
         const int cn = m - c0 < chunk ? m - c0 : chunk;
-        int left = fast_redo ? 0 : -1;      // -1: exact pipeline for the whole sub-batch
-        if (fast_redo) {
-            rc = pf_run(ctx, stream, d_frames, cn, H0, W0, p, meas_cap, rw, pools, nullptr, true, w.sel_idx + c0, nullptr, ctx->h_flags + 1, &rin);
-            if (rc != EPID_OK) return rc;
-            k_pf_compose_sel<<<1, 64, 0, stream>>>(rw.sel_idx, rw.counters, w.sel_idx + c0);
-            ctx->launches++;
-            EPID_CUDA(cudaStreamSynchronize(stream));      // the host needs the number of frames that were deferred again
-            left = ctx->h_flags[1];
-        } else {
-            rc = pf_run(ctx, stream, d_frames, cn, H0, W0, p, meas_cap, rw, pools, nullptr, false, w.sel_idx + c0);
-            if (rc != EPID_OK) return rc;
-            ctx->pf_exact_frames += cn;
-        }
+        rc = pf_run(ctx, stream, d_frames, cn, H0, W0, p, meas_cap, rw, pools, nullptr, true, w.sel_idx + c0, nullptr, ctx->h_flags + 1, &rin);
+        if (rc != EPID_OK) return rc;
+        k_pf_compose_sel<<<1, 64, 0, stream>>>(rw.sel_idx, rw.counters, w.sel_idx + c0);
+        ctx->launches++;
+        EPID_CUDA(cudaStreamSynchronize(stream));      // the host needs the number of frames that were deferred again
+        const int left = ctx->h_flags[1];
         if (!waited) { EPID_CUDA(cudaStreamWaitEvent(stream, after, 0)); waited = true; }
         k_pf_scatter_results<<<cn, 256, 0, stream>>>(w.sel_idx + c0, cn, rw.summ, rw.meas, w.summ, w.meas, meas_cap);
         ctx->launches++;
@@ -970,55 +955,6 @@ struct PfResultCopy {   // async D2H of one chunk's results + the counters ([2] 
 
 }  // namespace
 
-// S sub-batches on S streams (EPID_OPT_PF_SPLIT): every sub-batch is a complete, independent pipeline with its own work area, so the
-// results are those of the single-stream run; the streams fork from and join into ctx->stream.
-struct PfSplit {
-    int S = 0;
-    PfWork w[4];
-    int n0[4], nn[4];
-    cudaStream_t st[4];
-    cudaEvent_t fork = nullptr, join[4] = {nullptr, nullptr, nullptr, nullptr};
-    int prepare(epid_ctx* ctx, int n, int H, int W, int meas_cap) {
-        S = ctx->pf_split < n ? ctx->pf_split : n;
-        if (S < 2) { S = 0; return EPID_OK; }
-        size_t tot = 0, off[4];
-        for (int k = 0; k < S; k++) {
-            n0[k] = (int)((long long)n * k / S);
-            nn[k] = (int)((long long)n * (k + 1) / S) - n0[k];
-            carve(w[k], nullptr, nn[k], H, W, meas_cap);
-            off[k] = tot;
-            tot += align_up(w[k].total, 512);
-        }
-        int rc = ensure_scratch(ctx, tot);
-        if (rc != EPID_OK) return rc;
-        for (int k = 0; k < S; k++) carve(w[k], (char*)ctx->scratch + off[k], nn[k], H, W, meas_cap);
-        st[0] = ctx->stream;
-        for (int k = 1; k < S; k++) {
-            if (!ctx->aux_stream[k]) EPID_CUDA(cudaStreamCreateWithFlags(&ctx->aux_stream[k], cudaStreamNonBlocking));
-            st[k] = ctx->aux_stream[k];
-        }
-        EPID_CUDA(cudaEventCreateWithFlags(&fork, cudaEventDisableTiming));
-        for (int k = 1; k < S; k++) EPID_CUDA(cudaEventCreateWithFlags(&join[k], cudaEventDisableTiming));
-        return EPID_OK;
-    }
-    int do_fork(epid_ctx* ctx) {
-        EPID_CUDA(cudaEventRecord(fork, ctx->stream));
-        for (int k = 1; k < S; k++) EPID_CUDA(cudaStreamWaitEvent(st[k], fork, 0));
-        return EPID_OK;
-    }
-    int do_join(epid_ctx* ctx) {
-        for (int k = 1; k < S; k++) {
-            EPID_CUDA(cudaEventRecord(join[k], st[k]));
-            EPID_CUDA(cudaStreamWaitEvent(ctx->stream, join[k], 0));
-        }
-        return EPID_OK;
-    }
-    void destroy() {
-        if (fork) cudaEventDestroy(fork);
-        for (int k = 1; k < 4; k++) if (join[k]) cudaEventDestroy(join[k]);
-    }
-};
-
 extern "C" {
 
 int32_t epid_pf_analyze(epid_ctx* ctx, const epid_batch* frames, const epid_pf_params* p, epid_pf_summary* summary,
@@ -1035,62 +971,20 @@ int32_t epid_pf_analyze(epid_ctx* ctx, const epid_batch* frames, const epid_pf_p
     if (rc != EPID_OK) return rc;
     carve(w, (char*)ctx->scratch, n, H, W, meas_cap);
     uint16_t* pools[3] = {nullptr, nullptr, nullptr};
-    const bool fast = pf_fast_ok(ctx, p, frames->h, frames->w);
-    auto copy_and_wait = [&](int* cnt3) -> int {
-        int r = PfResultCopy::enqueue(ctx->stream, w, n, meas_cap, summary, meas, cnt3);
-        cudaError_t e = cudaStreamSynchronize(ctx->stream);
-        if (r == EPID_OK && e != cudaSuccess) { set_error("PF pipeline failed: %s", cudaGetErrorString(e)); r = EPID_ERR_CUDA; }
-        return r;
-    };
-    int cnt3[3] = {0, 0, 0};
-    if (fast && ctx->pf_split >= 2 && n >= 2 * ctx->pf_split) {
-        // sub-batches on several streams, each with its own work area; result rows are copied per sub-batch.  A sub-batch with
-        // deferred frames makes the call fall back to the single-stream path below (rare: noisy / undecidable frames).
-        PfSplit sp;
-        rc = sp.prepare(ctx, n, H, W, meas_cap);
-        bool deferred = false;
-        if (rc == EPID_OK && sp.S >= 2) {
-            const size_t per = (size_t)frames->h * frames->w;
-            rc = sp.do_fork(ctx);
-            int cnt[4][3] = {};
-            for (int k = 0; k < sp.S && rc == EPID_OK; k++) {
-                rc = pf_run(ctx, sp.st[k], (const uint16_t*)frames->dptr + per * sp.n0[k], sp.nn[k], frames->h, frames->w, p, meas_cap, sp.w[k],
-                            pools, nullptr, true);
-                if (rc == EPID_OK) rc = PfResultCopy::enqueue(sp.st[k], sp.w[k], sp.nn[k], meas_cap, summary + sp.n0[k], meas + (size_t)sp.n0[k] * meas_cap, cnt[k]);
-            }
-            if (rc == EPID_OK) rc = sp.do_join(ctx);
-            cudaError_t e = cudaStreamSynchronize(ctx->stream);
-            for (int k = 1; k < sp.S; k++) cudaStreamSynchronize(sp.st[k]);
-            if (rc == EPID_OK && e != cudaSuccess) { set_error("PF pipeline failed: %s", cudaGetErrorString(e)); rc = EPID_ERR_CUDA; }
-            for (int k = 0; k < sp.S; k++) deferred = deferred || cnt[k][2] > 0;
-        }
-        sp.destroy();
-        if (rc != EPID_OK || (sp.S >= 2 && !deferred)) {
-            for (int k = 0; k < 3; k++) if (pools[k]) cudaFree(pools[k]);
-            return rc;
-        }
-        rc = ensure_scratch(ctx, w.total);
-        if (rc != EPID_OK) return rc;
-        carve(w, (char*)ctx->scratch, n, H, W, meas_cap);
-    }
-    if (fast && ctx->pf_overlap_redo) {
-        // the re-run of deferred frames (if any) overlaps the window stages of the batch on ctx->redo_stream
+    const uint16_t* d_frames = (const uint16_t*)frames->dptr;
+    if (pf_fast_ok(ctx, p, frames->h, frames->w)) {
+        // frames the certified front end deferred (noise candidates, undecidable orientation) are re-run on ctx->redo_stream while
+        // the window stages of the batch run
         int m = 0;
-        rc = pf_run_overlapped(ctx, ctx->stream, (const uint16_t*)frames->dptr, n, frames->h, frames->w, p, meas_cap, w, pools, nullptr, &m);
+        rc = pf_run_overlapped(ctx, ctx->stream, d_frames, n, frames->h, frames->w, p, meas_cap, w, pools, nullptr, &m);
         if (m > 0) ctx->pf_fallbacks++;
-        if (rc == EPID_OK) rc = copy_and_wait(cnt3); else cudaStreamSynchronize(ctx->stream);
-        for (int k = 0; k < 3; k++) if (pools[k]) cudaFree(pools[k]);
-        return rc;
+    } else {
+        rc = pf_run(ctx, ctx->stream, d_frames, n, frames->h, frames->w, p, meas_cap, w, pools, nullptr, false);
     }
-    rc = pf_run(ctx, ctx->stream, (const uint16_t*)frames->dptr, n, frames->h, frames->w, p, meas_cap, w, pools, nullptr, fast);
-    if (rc == EPID_OK) rc = copy_and_wait(cnt3); else cudaStreamSynchronize(ctx->stream);
-    if (rc == EPID_OK && fast && cnt3[2] > 0) {
-        // frames the certified front end deferred (noise candidates, undecidable orientation): exactly those are re-run
-        ctx->pf_fallbacks++;
-        int dummy[3];
-        rc = pf_redo_deferred(ctx, ctx->stream, (const uint16_t*)frames->dptr, cnt3[2], frames->h, frames->w, p, meas_cap, w, pools);
-        if (rc == EPID_OK) rc = copy_and_wait(dummy); else cudaStreamSynchronize(ctx->stream);
-    }
+    int cnt3[3] = {0, 0, 0};
+    if (rc == EPID_OK) rc = PfResultCopy::enqueue(ctx->stream, w, n, meas_cap, summary, meas, cnt3);
+    cudaError_t e = cudaStreamSynchronize(ctx->stream);
+    if (rc == EPID_OK && e != cudaSuccess) { set_error("PF pipeline failed: %s", cudaGetErrorString(e)); rc = EPID_ERR_CUDA; }
     for (int k = 0; k < 3; k++) if (pools[k]) cudaFree(pools[k]);
     return rc;
 }
@@ -1115,48 +1009,8 @@ static int32_t pf_bench_impl(epid_ctx* ctx, const epid_batch* frames, const epid
     cudaEvent_t t0, t1;
     EPID_CUDA(cudaEventCreate(&t0));
     EPID_CUDA(cudaEventCreate(&t1));
-    if (fast && ctx->pf_split >= 2 && n >= 2 * ctx->pf_split && !stage_ms) {
-        // sub-batches on several streams; falls through to the single-stream path when a frame was deferred
-        PfSplit sp;
-        rc = sp.prepare(ctx, n, H, W, meas_cap);
-        bool deferred = false;
-        if (rc == EPID_OK && sp.S >= 2) {
-            const int64_t l0 = ctx->launches;
-            const size_t per = (size_t)frames->h * frames->w;
-            EPID_CUDA(cudaStreamSynchronize(ctx->stream));
-            EPID_CUDA(cudaEventRecord(t0, ctx->stream));
-            rc = sp.do_fork(ctx);
-            for (int it = 0; it < iters && rc == EPID_OK; it++)
-                for (int k = 0; k < sp.S && rc == EPID_OK; k++)
-                    rc = pf_run(ctx, sp.st[k], (const uint16_t*)frames->dptr + per * sp.n0[k], sp.nn[k], frames->h, frames->w, p, meas_cap, sp.w[k],
-                                pools, nullptr, true);
-            if (rc == EPID_OK) rc = sp.do_join(ctx);
-            cudaEventRecord(t1, ctx->stream);
-            int cnt[4][3] = {};
-            for (int k = 0; k < sp.S; k++) cudaMemcpyAsync(cnt[k], sp.w[k].counters, sizeof(cnt[k]), cudaMemcpyDeviceToHost, ctx->stream);
-            cudaStreamSynchronize(ctx->stream);
-            for (int k = 1; k < sp.S; k++) cudaStreamSynchronize(sp.st[k]);
-            for (int k = 0; k < sp.S; k++) deferred = deferred || cnt[k][2] > 0;
-            float ms = 0;
-            cudaEventElapsedTime(&ms, t0, t1);
-            if (total_ms) *total_ms = ms;
-            if (stats_kernel_ms) *stats_kernel_ms = 0.f;
-            if (launches) *launches = ctx->launches - l0;
-            if (redone) *redone = 0;
-        }
-        sp.destroy();
-        if (rc != EPID_OK || (sp.S >= 2 && !deferred)) {
-            cudaEventDestroy(t0); cudaEventDestroy(t1);
-            for (int k = 0; k < 3; k++) if (pools[k]) cudaFree(pools[k]);
-            return rc;
-        }
-        // carve() above re-used the scratch: restore the single-batch work area
-        rc = ensure_scratch(ctx, w.total);
-        if (rc != EPID_OK) return rc;
-        carve(w, (char*)ctx->scratch, n, H, W, meas_cap);
-    }
     // pass 0: back-to-back passes, no host round trip (what an ordinary batch costs).  If that left deferred frames, pass 1 times
-    // the real control flow: after every fast pass the host reads the deferred count and enqueues the per-frame exact re-run.
+    // the real control flow: after every fast pass the host reads the deferred count and enqueues the per-frame re-run.
     for (int mode = 0; mode < 2; mode++) {
         PfTimers tm;
         tm.on = true;
@@ -1166,16 +1020,10 @@ static int32_t pf_bench_impl(epid_ctx* ctx, const epid_batch* frames, const epid
         EPID_CUDA(cudaStreamSynchronize(ctx->stream));
         EPID_CUDA(cudaEventRecord(t0, ctx->stream));
         for (int it = 0; it < iters && rc == EPID_OK; it++) {
-            if (mode == 1 && ctx->pf_overlap_redo) {
+            if (mode == 1)
                 rc = pf_run_overlapped(ctx, ctx->stream, (const uint16_t*)frames->dptr, n, frames->h, frames->w, p, meas_cap, w, pools, &tm, nullptr);
-                continue;
-            }
-            rc = pf_run(ctx, ctx->stream, (const uint16_t*)frames->dptr, n, frames->h, frames->w, p, meas_cap, w, pools, &tm, fast);
-            if (mode == 1 && rc == EPID_OK) {
-                cudaMemcpyAsync(cnt3, w.counters, sizeof(cnt3), cudaMemcpyDeviceToHost, ctx->stream);
-                cudaStreamSynchronize(ctx->stream);
-                if (cnt3[2] > 0) rc = pf_redo_deferred(ctx, ctx->stream, (const uint16_t*)frames->dptr, cnt3[2], frames->h, frames->w, p, meas_cap, w, pools);
-            }
+            else
+                rc = pf_run(ctx, ctx->stream, (const uint16_t*)frames->dptr, n, frames->h, frames->w, p, meas_cap, w, pools, &tm, fast);
         }
         cudaEventRecord(t1, ctx->stream);
         if (mode == 0) cudaMemcpyAsync(cnt3, w.counters, sizeof(cnt3), cudaMemcpyDeviceToHost, ctx->stream);
@@ -1325,7 +1173,7 @@ int32_t epid_pf_analyze_host(epid_ctx* ctx, const uint16_t* frames, int32_t n, i
         if (fast && h_cnt[s][2] > 0) {     // re-run exactly the frames the front end deferred, then fetch the chunk's rows again
             ctx->pf_fallbacks++;
             // on the re-run stream: the chunk's own pass has finished, the next chunk's pass keeps ctx->stream busy meanwhile
-            cudaStream_t rs = ctx->pf_overlap_redo ? ctx->redo_stream : ctx->stream;
+            cudaStream_t rs = ctx->redo_stream;
             int r = pf_redo_deferred(ctx, rs, bufs[s], h_cnt[s][2], h, w_, p, meas_cap, works[s], pools);
             if (r != EPID_OK) return r;
             r = PfResultCopy::enqueue(rs, works[s], cnt, meas_cap, direct ? summary + (size_t)ci * chunk : h_summ[s],

@@ -14,8 +14,6 @@
 // a frame share one value; that is detected exactly (the decoded bin total then differs from the pixel count)
 // and the frame is re-run by the MODE 1 variant (32-bit counters over value>>1 plus a second pass resolving
 // the low bit), so results are always exact.
-#include <cstdlib>
-
 #include "stats.cuh"
 
 namespace epid {
@@ -860,9 +858,7 @@ static size_t stats_smem_bytes(const StatsGeom& g) {
 int launch_frame_stats(epid_ctx* ctx, cudaStream_t stream, const StatsGeom& g, const FrameRef* d_frames,
                        const int* d_out_index, int n, FrameStats* d_stats, uint32_t* d_rowsum, uint32_t* d_colsum) {
     // multi-CTA histogram path for every view it covers (d_out_index is not used by any caller of that path)
-    static int v1 = -1;
-    if (v1 < 0) { const char* e = getenv("EPID_STATS_V1"); v1 = e ? atoi(e) : 0; }
-    if (!v1 && !d_out_index && g.W <= 2040 && g.nranks <= STATS_MAX_RANKS)
+    if (!d_out_index && g.W <= 2040 && g.nranks <= STATS_MAX_RANKS)
         return launch_frame_stats_v2(ctx, stream, g, d_frames, n, d_stats, d_rowsum, d_colsum);
     const size_t smem = stats_smem_bytes(g);
     EPID_SMEM_OPT_IN(ctx, k_frame_stats<0>, 220 * 1024);

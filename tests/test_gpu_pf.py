@@ -205,6 +205,21 @@ def test_fast_front_kernel_equals_exact_pipeline(name):
                 np.testing.assert_array_equal(exact.meas[k][i, :m], fast.meas[k][i, :m], err_msg=k)
 
 
+def test_set_option_rejects_unknown_keys():
+    """The options keep their numbers (EPID_OPT_PF_EXACT_ONLY = 1, EPID_OPT_PF_WIN2 = 3, EPID_OPT_STATS_EXACT = 7); any other key is
+    refused with EPID_ERR_INVALID (ValueError) rather than silently ignored."""
+    from pylinac_b200 import _native as nat
+
+    ctx = nat.Context.default()
+    assert (nat.OPT_PF_EXACT_ONLY, nat.OPT_PF_WIN2, nat.OPT_STATS_EXACT) == (1, 3, 7)
+    for key, default in ((1, 0), (3, 1), (7, 0)):
+        ctx.set_option(key, default)
+    for key in (0, 2, 4, 5, 6, 8):
+        assert nat.lib().epid_set_option(ctx.handle, key, 1) == nat.ERR_INVALID, key
+        with pytest.raises(ValueError, match=f"unknown option {key}"):
+            ctx.set_option(key, 1)
+
+
 def test_fast_front_kernel_is_used_for_the_benchmark_frames():
     from oracle import synth
     from pylinac_b200 import _native as nat
@@ -284,7 +299,7 @@ def test_pf_degenerate_inputs_fail_like_the_reference():
         pf.analyze_batch(np.zeros((1, 1024, 1024), np.float32), 2.56)
 
 
-def _leafband_cases():
+def _window_cases():
     from oracle import synth
     from tests.golden import pf_docs_cases as dc
 
@@ -310,49 +325,6 @@ def _leafband_cases():
             fr, ps, sid, ak = dc.docs_frame(nm)
             out["docs_" + nm] = (fr[None], (1 / ps) * sid / 1000.0, ak)
     return out
-
-
-@pytest.mark.parametrize("name", list(_leafband_cases()))
-def test_leafband_kernel_equals_per_window_kernel(name):
-    """The experimental leaf-band window kernel (one CTA per leaf, all pickets at once; opt-in, see DESIGN.md 4.6) must reproduce
-    the per-window kernel bit for bit."""
-    from pylinac_b200 import _native as nat
-    from pylinac_b200 import picketfence as pf
-
-    frames, dpmm, kw = _leafband_cases()[name]
-    ctx = nat.Context.default()
-    try:
-        ctx.set_option(nat.OPT_PF_LEAFBAND, 0)
-        old = pf.analyze_batch(frames, dpmm, **kw)
-        ctx.set_option(nat.OPT_PF_LEAFBAND, 1)
-        new = pf.analyze_batch(frames, dpmm, **kw)
-    finally:
-        ctx.set_option(nat.OPT_PF_LEAFBAND, 0)
-    for k in old.summary.dtype.names:
-        np.testing.assert_array_equal(old.summary[k], new.summary[k], err_msg=k)
-    for i in range(len(frames)):
-        if int(old.summary["status"][i]) == 0:
-            m = int(old.summary["n_meas"][i])
-            assert m > 0
-            for k in old.meas.dtype.names:
-                np.testing.assert_array_equal(old.meas[k][i, :m], new.meas[k][i, :m], err_msg=k)
-
-
-def test_leafband_kernel_runs_when_enabled():
-    from oracle import synth
-    from pylinac_b200 import _native as nat
-    from pylinac_b200 import picketfence as pf
-
-    ctx = nat.Context.default()
-    frames = np.stack([synth.bench_pf_frame(i) for i in range(60, 76)])
-    b = nat.Batch.upload(ctx, frames)
-    try:
-        ctx.set_option(nat.OPT_PF_LEAFBAND, 1)
-        st = nat.pf_bench_stages(ctx, b, pf.make_params(2.56, frames.shape[1:]), 2)
-    finally:
-        ctx.set_option(nat.OPT_PF_LEAFBAND, 0)
-        b.free()
-    assert st["k_pf_leafband"] > 5 * st["k_pf_windows_fast"] > 0
 
 
 def test_pf_host_pipeline_staged_and_direct_result_paths_agree():
@@ -383,14 +355,14 @@ def test_pf_host_pipeline_staged_and_direct_result_paths_agree():
             np.testing.assert_array_equal(m_direct[k][i, :m], m_staged[k][i, :m], err_msg=k)
 
 
-@pytest.mark.parametrize("name", list(_leafband_cases()))
+@pytest.mark.parametrize("name", list(_window_cases()))
 def test_two_kernel_window_path_equals_per_window_kernel(name):
     """The default window path (k_pf_win_medians + k_pf_win_fwxm, pf_windows2.cu) must reproduce the single per-window kernel
     (k_pf_windows_fast, pinned to the reference by the golden tests) bit for bit, on frames it covers and on frames it declines."""
     from pylinac_b200 import _native as nat
     from pylinac_b200 import picketfence as pf
 
-    frames, dpmm, kw = _leafband_cases()[name]
+    frames, dpmm, kw = _window_cases()[name]
     ctx = nat.Context.default()
     try:
         ctx.set_option(nat.OPT_PF_WIN2, 0)
@@ -519,11 +491,11 @@ def _assert_same_results(a, b):
             np.testing.assert_array_equal(ma[k][i, :m], mb[k][i, :m], err_msg=f"{k} frame {i}")
 
 
-def test_pf_certified_noise_rerun_equals_the_exact_rerun_and_overlaps():
+def test_pf_certified_noise_rerun_equals_the_exact_pipeline():
     """The per-frame fallback: frames whose _has_noise() the single exact count certifies are median filtered and re-run by the
-    certified fast pipeline (frames with a hot block are deferred again -> exact pipeline).  Every variant -- fast / exact re-run,
-    overlapped on the second stream or serial, device-resident or host entry point -- must return bit-identical rows, and the hot-pixel
-    frames must equal the oracle."""
+    certified fast pipeline on the second stream, overlapped with the batch's window stages (frames with a hot block are deferred
+    again -> exact pipeline).  The device-resident and the host entry point must both return the rows of the exact-histogram
+    pipeline run on every frame (OPT_PF_EXACT_ONLY) bit for bit, and the hot-pixel frames must equal the oracle."""
     from oracle import pf_oracle
     from pylinac_b200 import _native as nat
     from pylinac_b200 import picketfence as pf
@@ -532,30 +504,23 @@ def test_pf_certified_noise_rerun_equals_the_exact_rerun_and_overlaps():
     ctx = nat.Context.default()
     params = pf.make_params(2.56, frames.shape[1:])
     b = nat.Batch.upload(ctx, frames)
-    results = {}
-    counts = {}
     try:
-        for fast_redo in (1, 0):
-            for overlap in (1, 0):
-                ctx.set_option(nat.OPT_PF_FAST_REDO, fast_redo)
-                ctx.set_option(nat.OPT_PF_OVERLAP_REDO, overlap)
-                r0, e0 = ctx.counter(nat.CTR_PF_REDONE_FRAMES), ctx.counter(nat.CTR_PF_EXACT_FRAMES)
-                results[(fast_redo, overlap, "dev")] = nat.pf_analyze(ctx, b, params)
-                counts[(fast_redo, overlap)] = (ctx.counter(nat.CTR_PF_REDONE_FRAMES) - r0, ctx.counter(nat.CTR_PF_EXACT_FRAMES) - e0)
-                s, m = nat.pf_analyze(ctx, frames, params)
-                results[(fast_redo, overlap, "host")] = (s.copy(), m.copy())
+        ctx.set_option(nat.OPT_PF_EXACT_ONLY, 1)
+        ref = nat.pf_analyze(ctx, b, params)
+        ctx.set_option(nat.OPT_PF_EXACT_ONLY, 0)
+        r0, e0 = ctx.counter(nat.CTR_PF_REDONE_FRAMES), ctx.counter(nat.CTR_PF_EXACT_FRAMES)
+        dev = nat.pf_analyze(ctx, b, params)
+        counts = (ctx.counter(nat.CTR_PF_REDONE_FRAMES) - r0, ctx.counter(nat.CTR_PF_EXACT_FRAMES) - e0)
+        s, m = nat.pf_analyze(ctx, frames, params)
+        host = (s.copy(), m.copy())
     finally:
-        ctx.set_option(nat.OPT_PF_FAST_REDO, 1)
-        ctx.set_option(nat.OPT_PF_OVERLAP_REDO, 1)
+        ctx.set_option(nat.OPT_PF_EXACT_ONLY, 0)
         b.free()
     n_hot, n_block = kinds.count("hot"), kinds.count("block")
     assert n_hot >= 8 and n_block >= 4
-    for overlap in (1, 0):
-        assert counts[(1, overlap)] == (n_hot + n_block, n_block), counts      # only the hot-block frames need the exact pipeline
-        assert counts[(0, overlap)] == (n_hot + n_block, n_hot + n_block), counts
-    ref = results[(0, 0, "dev")]
-    for key, val in results.items():
-        _assert_same_results(ref, val)
+    assert counts == (n_hot + n_block, n_block), counts      # only the hot-block frames need the exact pipeline
+    _assert_same_results(ref, dev)
+    _assert_same_results(ref, host)
     s, m = ref
     assert np.all(s["status"] == 0)
     for i, kind in enumerate(kinds):
