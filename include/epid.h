@@ -629,6 +629,28 @@ enum {
 int32_t epid_xim_decode(epid_ctx* ctx, const void* arena, size_t arena_bytes, const int64_t* desc, int32_t n, int32_t h, int32_t w,
                         int32_t bpp, int32_t dtype, int32_t* status, epid_batch** out);
 
+/* ----------------------------------------------------------------------------------------- machine-log fluence
+ * FluenceBase.calc_map(resolution, equal_aspect) (log_analyzer.py:478-612) for a batch of n trajectory logs / Dynalogs, actual
+ * (kinds bit 0) and expected (bit 1) in one launch sequence.  `arena` (host, page-locked for a DMA copy) holds every log's column
+ * table; logs: n descriptors of 88 bytes (pylinac_b200/log_analyzer.py LOG_DESC_DTYPE, csrc/logs.cu LogDesc): byte offset,
+ * snapshot / column strides, element size (float32 trajectory-log body or float64 Dynalog columns), the MU / jaw X1 / X2 / leaf
+ * columns, the slice of `snaps` holding the beam-on snapshot indices, the slice of `pair_flags` (bit 0: pair under a Y jaw,
+ * MLC.leaf_under_y_jaw :1260-1290; bit 1: pair moved, MLC.pair_moved :1002-1016), the slice of `rows` ([start, stop) output
+ * rows per pair, from the reference's int cast of the leaf-width cumsum) and per kind bit 0 "map stays zero" (no beam-on
+ * snapshot, max(MU) < 0.5) and bit 1 "divide by MU_total" (MU_total == 25000, :608-610).  out_*: float64 batches [n][h][w]
+ * (w = int(400 / resolution)); a kind not requested is returned as NULL.  Bit-identical to the reference: float32 line, double
+ * rounding per snapshot, round-half-even edges, numpy slice semantics. */
+int32_t epid_log_fluence(epid_ctx* ctx, const void* arena, size_t arena_bytes, const void* logs, int32_t n, const int32_t* snaps,
+                         int32_t n_snaps, const uint8_t* pair_flags, int32_t n_pair_flags, const int32_t* rows, int32_t n_rows,
+                         double resolution, int32_t w, int32_t h, int32_t kinds, epid_batch** out_actual, epid_batch** out_expected);
+/* BaseImage.check_inversion_by_histogram() (core/image.py:899-926) of float64 frames: np.percentile(a, 5 / 50 / 95) from exact order
+ * statistics (radix select), and where |p50 - p5| > |p50 - p95| the frame is inverted (-a + max + min, core/array_utils.py:75-77).
+ * out: a new float64 batch; inverted (host, int32 [n], may be NULL): the per-frame decision.  Frames must hold no nan. */
+int32_t epid_hist_invert(epid_ctx* ctx, const epid_batch* in, epid_batch** out, int32_t* inverted);
+/* GammaFluence.calc_map statistics (log_analyzer.py:743-748) per frame of a float64 gamma batch: sum and count of the non-nan
+ * values and the count below 1 (host: avg_gamma = sum / count or 0, pass_prcnt = passing / count * 100).  Outputs are host arrays [n]. */
+int32_t epid_gamma_stats(epid_ctx* ctx, const epid_batch* gamma, double* sum, int64_t* count, int64_t* passing);
+
 /* ----------------------------------------------------------------------------------------- multi-GPU (NCCL)
  * The batch shards by frame index with no data-path collective; the only exchange is the final gather of the
  * fixed-size per-frame result structs (SURVEY.md 8e).  id: 128-byte ncclUniqueId created by rank 0. */

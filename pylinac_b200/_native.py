@@ -330,6 +330,10 @@ _SIGNATURES = {
     "epid_gather_results": [_P, _P, C.c_size_t, _P],
     "epid_barrier": [_P],
     "epid_xim_decode": [_P, _P, C.c_size_t, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P, C.POINTER(_P)],
+    "epid_log_fluence": [_P, _P, C.c_size_t, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_double, C.c_int32,
+                         C.c_int32, C.c_int32, C.POINTER(_P), C.POINTER(_P)],
+    "epid_hist_invert": [_P, _P, C.POINTER(_P), _P],
+    "epid_gamma_stats": [_P, _P, _P, _P, _P],
 }
 
 
@@ -572,6 +576,46 @@ def xim_decode(ctx: Context, arena: np.ndarray, desc: np.ndarray, h: int, w: int
     check(lib().epid_xim_decode(ctx.handle, _ptr(a), a.nbytes, _ptr(d), len(d), int(h), int(w), int(bpp), _NP2DT[np.dtype(dtype)],
                                 _ptr(status), C.byref(h_out)))
     return Batch(ctx, h_out), status
+
+
+LOG_DESC_DTYPE = np.dtype([("data_off", "<i8"), ("snap_stride", "<i8"), ("col_stride", "<i8"), ("f64", "<i4"), ("nsnap", "<i4"),
+                           ("col_mu", "<i4", (2,)), ("col_x1", "<i4"), ("col_x2", "<i4"), ("col_leaf", "<i4", (2,)), ("num_pairs", "<i4"),
+                           ("snap_off", "<i4"), ("nbeam", "<i4"), ("pair_off", "<i4"), ("row_off", "<i4"), ("flags", "<i4", (2,)),
+                           ("pad", "<i4")])
+assert LOG_DESC_DTYPE.itemsize == 88
+LF_ZERO, LF_DIV25000 = 1, 2
+PF_UNDER_JAW, PF_MOVED = 1, 2
+
+
+def log_fluence(ctx: Context, arena: np.ndarray, logs: np.ndarray, snaps: np.ndarray, pair_flags: np.ndarray, rows: np.ndarray,
+                resolution: float, w: int, h: int, kinds: int = 3) -> tuple[Batch | None, Batch | None]:
+    """epid_log_fluence -> (actual, expected) float64 device batches [n, h, w] (None for a kind not requested)"""
+    a = np.ascontiguousarray(arena).view(np.uint8).reshape(-1)
+    d = np.ascontiguousarray(logs, dtype=LOG_DESC_DTYPE)
+    s = np.ascontiguousarray(snaps, dtype=np.int32)
+    pf = np.ascontiguousarray(pair_flags, dtype=np.uint8)
+    r = np.ascontiguousarray(rows, dtype=np.int32)
+    ha, he = _P(), _P()
+    check(lib().epid_log_fluence(ctx.handle, _ptr(a), a.nbytes, _ptr(d), len(d), _ptr(s) if s.size else None, s.size, _ptr(pf), pf.size,
+                                 _ptr(r), r.size, float(resolution), int(w), int(h), int(kinds), C.byref(ha), C.byref(he)))
+    return (Batch(ctx, ha) if ha.value else None), (Batch(ctx, he) if he.value else None)
+
+
+def hist_invert(ctx: Context, batch: Batch) -> tuple[Batch, np.ndarray]:
+    """epid_hist_invert: check_inversion_by_histogram of every float64 frame -> (new batch, int32 inverted [n])"""
+    (n, _, _), _ = batch.shape_dtype
+    inv = np.zeros(n, np.int32)
+    h = _P()
+    check(lib().epid_hist_invert(ctx.handle, batch.handle, C.byref(h), _ptr(inv)))
+    return Batch(ctx, h), inv
+
+
+def gamma_stats(ctx: Context, gamma: Batch) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """epid_gamma_stats -> (sum of non-nan values, their count, count below 1) per frame"""
+    (n, _, _), _ = gamma.shape_dtype
+    s, c, p = np.zeros(n), np.zeros(n, np.int64), np.zeros(n, np.int64)
+    check(lib().epid_gamma_stats(ctx.handle, gamma.handle, _ptr(s), _ptr(c), _ptr(p)))
+    return s, c, p
 
 
 def frame_stats(ctx: Context, batch: Batch, view=None, percentiles=()):
