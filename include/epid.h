@@ -651,6 +651,19 @@ int32_t epid_hist_invert(epid_ctx* ctx, const epid_batch* in, epid_batch** out, 
  * values and the count below 1 (host: avg_gamma = sum / count or 0, pass_prcnt = passing / count * 100).  Outputs are host arrays [n]. */
 int32_t epid_gamma_stats(epid_ctx* ctx, const epid_batch* gamma, double* sum, int64_t* count, int64_t* passing);
 
+/* ----------------------------------------------------------------------------------------- CT stacks (WinstonLutz.from_cbct)
+ * epid_stack_mip: the two maximum-intensity projections of winston_lutz.py:1465-1489 for a volume [N][H][W] of slices in sorted
+ * order (I16 or U16; other dtypes EPID_ERR_UNSUPPORTED, as are slices wider than 2048 pixels): np.stack(images, axis=-1).max(axis=0)
+ * -> colmax, a new batch [W][1][N], and .max(axis=1) -> rowmax [H][1][N], in the volume's dtype.  Each row is one 1-D signal, the
+ * layout epid_zoom takes to resample the slice axis.  One read of the volume; integer max, exact.
+ * epid_cbct_views: the four pseudo-cardinal frames of winston_lutz.py:1470-1505 from zoomed projections (epid_zoom output, float64
+ * [P][1][N']): for z0 (then z1, which may be NULL and must have z0's shape) frame 2 p = np.rot90(z, 1) and frame 2 p + 1 = its
+ * np.fliplr.  Values are rounded like scipy.ndimage.zoom's integer output of src_dtype (I16: half away from zero; U16: + 0.5; both
+ * clamped to the type) and stored as the 16 bits array_to_dicom writes (PixelRepresentation 0: int16 bits read back as uint16).
+ * out: a new U16 batch [2 or 4][N'][P]. */
+int32_t epid_stack_mip(epid_ctx* ctx, const epid_batch* volume, epid_batch** colmax, epid_batch** rowmax);
+int32_t epid_cbct_views(epid_ctx* ctx, const epid_batch* z0, const epid_batch* z1, int32_t src_dtype, epid_batch** out);
+
 /* ----------------------------------------------------------------------------------------- multi-GPU (NCCL)
  * The batch shards by frame index with no data-path collective; the only exchange is the final gather of the
  * fixed-size per-frame result structs (SURVEY.md 8e).  id: 128-byte ncclUniqueId created by rank 0. */

@@ -334,6 +334,8 @@ _SIGNATURES = {
                          C.c_int32, C.c_int32, C.POINTER(_P), C.POINTER(_P)],
     "epid_hist_invert": [_P, _P, C.POINTER(_P), _P],
     "epid_gamma_stats": [_P, _P, _P, _P, _P],
+    "epid_stack_mip": [_P, _P, C.POINTER(_P), C.POINTER(_P)],
+    "epid_cbct_views": [_P, _P, _P, C.c_int32, C.POINTER(_P)],
 }
 
 
@@ -616,6 +618,32 @@ def gamma_stats(ctx: Context, gamma: Batch) -> tuple[np.ndarray, np.ndarray, np.
     s, c, p = np.zeros(n), np.zeros(n, np.int64), np.zeros(n, np.int64)
     check(lib().epid_gamma_stats(ctx.handle, gamma.handle, _ptr(s), _ptr(c), _ptr(p)))
     return s, c, p
+
+
+def _unsupported_as_not_implemented(rc):
+    try:
+        check(rc)
+    except NativeError as e:
+        if e.code == ERR_UNSUPPORTED:
+            raise NotImplementedError(e.msg) from None
+        raise
+
+
+def stack_mip(ctx: Context, volume: Batch) -> tuple[Batch, Batch]:
+    """epid_stack_mip: volume [N, H, W] int16 / uint16 -> (colmax [W, 1, N], rowmax [H, 1, N]) device batches of the volume's dtype:
+    np.stack(slices, axis=-1).max(axis=0) / .max(axis=1).  Other dtypes raise NotImplementedError."""
+    hc, hr = _P(), _P()
+    _unsupported_as_not_implemented(lib().epid_stack_mip(ctx.handle, volume.handle, C.byref(hc), C.byref(hr)))
+    return Batch(ctx, hc), Batch(ctx, hr)
+
+
+def cbct_views(ctx: Context, z0: Batch, z1: Batch | None, src_dtype) -> Batch:
+    """epid_cbct_views: zoomed projections (float64 [P, 1, N']) -> uint16 frames [2 or 4, N', P]: rot90 and fliplr(rot90) of z0, then
+    of z1, rounded like scipy's integer zoom output of `src_dtype` and stored as the uint16 bits of that dtype."""
+    h = _P()
+    _unsupported_as_not_implemented(lib().epid_cbct_views(ctx.handle, z0.handle, None if z1 is None else z1.handle,
+                                                          _NP2DT[np.dtype(src_dtype)], C.byref(h)))
+    return Batch(ctx, h)
 
 
 def frame_stats(ctx: Context, batch: Batch, view=None, percentiles=()):

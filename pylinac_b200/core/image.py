@@ -461,20 +461,22 @@ class ArrayImage(BaseImage):
 
 
 class DicomImage(BaseImage):
-    """core/image.py:1383-1580 with pylinac_b200.dicom instead of pydicom."""
+    """core/image.py:1383-1580 with pylinac_b200.dicom instead of pydicom.  `path` may also be a ``dicom.Dataset`` already read
+    (with ``pixel_array`` set, as DicomImageStack builds its slices): the image then views those pixels instead of copying them."""
 
     def __init__(self, path, *, dtype=None, dpi: float = None, sid: float = None, sad: float = 1000, raw_pixels: bool = False,
                  invert_pixels: bool | None = None):
+        in_memory = isinstance(path, dicom.Dataset)
         super().__init__(path)
         self._sid = sid
         self._dpi = dpi
         self._sad = sad
-        self.metadata = dicom.dcmread(path)
+        self.metadata = path if in_memory else dicom.dcmread(path)
         pix = self.metadata.pixel_array
         self._original_dtype = pix.dtype
         self._raw_pixels = raw_pixels
         self._invert_pixels = invert_pixels
-        self.array = pix.astype(dtype) if dtype is not None else pix.copy()
+        self.array = pix.astype(dtype) if dtype is not None else (pix if in_memory else pix.copy())
         self.array = _rescale_dicom_values(self.array, self.metadata, raw_pixels, invert_pixels)
         # the stored integers + the map that produced ``array`` from them (frame_u16 analyses the stored values when the
         # array is still that map of them)
@@ -610,37 +612,8 @@ class LinacDicomImage(DicomImage):
     _AXIS_NAMES = {"gantry": "Gantry", "coll": "Coll", "couch": "Couch"}
 
     def _axis(self, key, tag):
-        """_get_axis_value (core/image.py:1655-1730): explicit value, else `<axis><number>` in the file name when use_filenames
-        (keyword absent -> missing_axis_value, the tags are not consulted), else the DICOM tag, else missing_axis_value."""
-        import os.path as osp
-        import re
-
-        name = self._AXIS_NAMES[key]
-        if key in self._axis_overrides and self._axis_overrides[key] is not None:
-            v = self._axis_overrides[key]
-        elif self._use_filenames:
-            filename = osp.basename(str(self.path)).lower()
-            if name.lower() not in filename:
-                if self._missing_axis_value == "raise":
-                    raise ValueError(f"{name} axis value was not found in the filename and `missing_axis_value` was `raise`. "
-                                     "Either provide an axis value or pass a numerical value for `missing_axis_value`.")
-                v = self._missing_axis_value
-            else:
-                m = re.search(rf"(?<={name.lower()})\d+", filename)
-                if m is None:
-                    raise ValueError(f"The filename contains '{name}' but could not read a number following it. "
-                                     f"Use the format '...{name}<#>...'")
-                v = float(m.group())
-        else:
-            v = self.metadata.get(tag)
-            if v is None:
-                if self._missing_axis_value == "raise":
-                    raise ValueError(f"Axis {key} was not found in the DICOM tags")
-                v = self._missing_axis_value
-        v = float(v)
-        if self._axes_precision is not None:
-            v = round(v, self._axes_precision)
-        return v % 360 if v >= 360 else v
+        return linac_axis_value(key, self._axis_overrides.get(key), self.path, self.metadata.get(tag), use_filenames=self._use_filenames,
+                                missing_axis_value=self._missing_axis_value, axes_precision=self._axes_precision)
 
     @property
     def gantry_angle(self) -> float:
@@ -653,6 +626,121 @@ class LinacDicomImage(DicomImage):
     @property
     def couch_angle(self) -> float:
         return self._axis("couch", "PatientSupportAngle")
+
+
+def linac_axis_value(key: str, override, path, tag_value, *, use_filenames: bool, missing_axis_value, axes_precision):
+    """_get_axis_value (core/image.py:1655-1730) of axis `key` ('gantry' / 'coll' / 'couch'): explicit value, else `<axis><number>`
+    in the file name when use_filenames (keyword absent -> missing_axis_value, the tags are not consulted), else the DICOM tag value,
+    else missing_axis_value."""
+    import re
+
+    name = LinacDicomImage._AXIS_NAMES[key]
+    if override is not None:
+        v = override
+    elif use_filenames:
+        filename = osp.basename(str(path)).lower()
+        if name.lower() not in filename:
+            if missing_axis_value == "raise":
+                raise ValueError(f"{name} axis value was not found in the filename and `missing_axis_value` was `raise`. "
+                                 "Either provide an axis value or pass a numerical value for `missing_axis_value`.")
+            v = missing_axis_value
+        else:
+            m = re.search(rf"(?<={name.lower()})\d+", filename)
+            if m is None:
+                raise ValueError(f"The filename contains '{name}' but could not read a number following it. "
+                                 f"Use the format '...{name}<#>...'")
+            v = float(m.group())
+    else:
+        v = tag_value
+        if v is None:
+            if missing_axis_value == "raise":
+                raise ValueError(f"Axis {key} was not found in the DICOM tags")
+            v = missing_axis_value
+    v = float(v)
+    if axes_precision is not None:
+        v = round(v, axes_precision)
+    return v % 360 if v >= 360 else v
+
+
+def _image_header(path):
+    """LazyDicomImageStack._get_path_metadatas (core/image.py:1952-1966) for one file: its header when its SOP Class UID names an
+    image storage class; None for a file that does not parse as DICOM, has no SOP Class UID or is not an image."""
+    try:
+        ds = dicom.read_header(path)
+        uid = ds.SOPClassUID
+    except OSError:
+        raise
+    except Exception:
+        return None
+    return ds if uid in dicom.IMAGE_STORAGE_UIDS else None
+
+
+class DicomImageStack:
+    """core/image.py:1873-2210 (LazyDicomImageStack.__init__ + DicomImageStack.__init__): the image files of a folder (searched
+    recursively; a list or tuple of paths is taken as given), filtered to the most common SeriesInstanceUID and sorted by the last
+    ImagePositionPatient coordinate.  Headers are parsed on a thread pool without touching pixel data, then every slice's pixels are
+    read in sorted order into one [n, rows, cols] page-locked array, ``volume``; ``images[i]`` is a DicomImage viewing
+    ``volume[i]`` (``dtype`` / ``raw_pixels`` applied as DicomImage applies them)."""
+
+    def __init__(self, folder, dtype=None, min_number: int = 39, check_uid: bool = True, raw_pixels: bool = False):
+        from collections import Counter
+        from concurrent.futures import ThreadPoolExecutor
+
+        self.dtype = dtype
+        paths = []
+        if isinstance(folder, (list, tuple)):
+            paths = [str(p) for p in folder]
+        elif osp.isdir(folder):
+            for pdir, _sdir, files in os.walk(folder):
+                for file in files:
+                    paths.append(osp.join(pdir, file))
+        with ThreadPoolExecutor(max(1, min(8, len(paths)))) as pool:
+            headers = list(pool.map(_image_header, paths))
+        metadatas = [h for h in headers if h is not None]
+        paths = [p for p, h in zip(paths, headers) if h is not None]
+        if len(paths) < 1:
+            raise FileNotFoundError(f"No files were found in the specified location: {folder}")
+        if check_uid:
+            most_common_uid = Counter(m.SeriesInstanceUID for m in metadatas).most_common(1)[0]
+            if most_common_uid[1] < min_number:
+                raise ValueError("The minimum number images from the same study were not found")
+            keep = [k for k, m in enumerate(metadatas) if m.SeriesInstanceUID == most_common_uid[0]]
+            metadatas, paths = [metadatas[k] for k in keep], [paths[k] for k in keep]
+        order = np.argsort([m.ImagePositionPatient[-1] for m in metadatas])
+        self.metadatas = [metadatas[i] for i in order]
+        self._image_path_keys = [paths[i] for i in order]
+        h0 = self.metadatas[0]
+        shape = (len(self.metadatas), int(h0["Rows"]), int(h0["Columns"]))
+        try:
+            volume = nat.pinned_empty(shape, h0["PixelDtype"])
+        except nat.NativeError:      # no CUDA device: pageable host memory (only the H2D copy is slower)
+            volume = None
+        self.volume, _ = dicom.read_frames(self._image_path_keys, out=volume, headers=self.metadatas)
+        for m, pixels in zip(self.metadatas, self.volume):
+            m.pixel_array = pixels
+        self.images = [DicomImage(m, dtype=dtype, raw_pixels=raw_pixels) for m in self.metadatas]
+
+    @classmethod
+    def from_zip(cls, zip_path, dtype=None, **kwargs):
+        """core/image.py:2167-2180"""
+        with TemporaryZipDirectory(zip_path) as tmpzip:
+            return cls(tmpzip, dtype, **kwargs)
+
+    @property
+    def metadata(self):
+        """The metadata of the first (sorted) slice."""
+        return self[0].metadata
+
+    @property
+    def slice_spacing(self) -> float:
+        """core/image.py:1983-1989: distance between the first two slices."""
+        return np.abs(self.metadatas[0].ImagePositionPatient[-1] - self.metadatas[1].ImagePositionPatient[-1])
+
+    def __getitem__(self, item) -> DicomImage:
+        return self.images[item]
+
+    def __len__(self):
+        return len(self.images)
 
 
 class XIM(BaseImage):

@@ -77,7 +77,7 @@ __global__ void k_zoom_eval(const double* __restrict__ c, int n, int Hp, int Wp,
             w[3] = 1.0 - w[0] - w[1] - w[2];
             *start = (int)fl - 1;
         } else {
-            w[0] = 1.0 - t; w[1] = t; w[2] = 0.0; w[3] = 0.0;
+            w[0] = 1.0 - t; w[1] = 1.0 - w[0]; w[2] = 0.0; w[3] = 0.0;      // scipy: the last weight is 1 - the others
             *start = (int)fl;
         }
     };

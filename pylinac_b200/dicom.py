@@ -25,8 +25,11 @@ _TAGS = {
     (0x0008, 0x0013): ("InstanceCreationTime", "str"),
     (0x0008, 0x0023): ("ContentDate", "str"),
     (0x0008, 0x0033): ("ContentTime", "str"),
+    (0x0018, 0x0050): ("SliceThickness", "ds"),
     (0x0018, 0x1110): ("DistanceSourceToDetector", "ds"),
     (0x0018, 0x1164): ("ImagerPixelSpacing", "ds"),
+    (0x0020, 0x000E): ("SeriesInstanceUID", "str"),
+    (0x0020, 0x0032): ("ImagePositionPatient", "ds"),
     (0x0028, 0x0002): ("SamplesPerPixel", "us"),
     (0x0028, 0x0008): ("NumberOfFrames", "is"),
     (0x0028, 0x0010): ("Rows", "us"),
@@ -48,6 +51,48 @@ _TAGS = {
     (0x300A, 0x0122): ("PatientSupportAngle", "ds"),
 }
 _PIXEL_DATA = (0x7FE0, 0x0010)
+
+# The standard storage SOP classes (DICOM PS3.6 annex A) whose names contain "Image Storage": LazyDicomImageStack keeps a file when
+# ``"Image Storage" in ds.SOPClassUID.name`` (core/image.py:1961); pydicom's UID names are restated here as a table.
+IMAGE_STORAGE_UIDS = {
+    "1.2.840.10008.5.1.4.1.1.1": "Computed Radiography Image Storage",
+    "1.2.840.10008.5.1.4.1.1.1.1": "Digital X-Ray Image Storage - For Presentation",
+    "1.2.840.10008.5.1.4.1.1.1.1.1": "Digital X-Ray Image Storage - For Processing",
+    "1.2.840.10008.5.1.4.1.1.1.2": "Digital Mammography X-Ray Image Storage - For Presentation",
+    "1.2.840.10008.5.1.4.1.1.1.2.1": "Digital Mammography X-Ray Image Storage - For Processing",
+    "1.2.840.10008.5.1.4.1.1.1.3": "Digital Intra-Oral X-Ray Image Storage - For Presentation",
+    "1.2.840.10008.5.1.4.1.1.1.3.1": "Digital Intra-Oral X-Ray Image Storage - For Processing",
+    "1.2.840.10008.5.1.4.1.1.2": "CT Image Storage",
+    "1.2.840.10008.5.1.4.1.1.2.1": "Enhanced CT Image Storage",
+    "1.2.840.10008.5.1.4.1.1.2.2": "Legacy Converted Enhanced CT Image Storage",
+    "1.2.840.10008.5.1.4.1.1.3.1": "Ultrasound Multi-frame Image Storage",
+    "1.2.840.10008.5.1.4.1.1.4": "MR Image Storage",
+    "1.2.840.10008.5.1.4.1.1.4.1": "Enhanced MR Image Storage",
+    "1.2.840.10008.5.1.4.1.1.4.3": "Enhanced MR Color Image Storage",
+    "1.2.840.10008.5.1.4.1.1.4.4": "Legacy Converted Enhanced MR Image Storage",
+    "1.2.840.10008.5.1.4.1.1.6.1": "Ultrasound Image Storage",
+    "1.2.840.10008.5.1.4.1.1.7": "Secondary Capture Image Storage",
+    "1.2.840.10008.5.1.4.1.1.7.1": "Multi-frame Single Bit Secondary Capture Image Storage",
+    "1.2.840.10008.5.1.4.1.1.7.2": "Multi-frame Grayscale Byte Secondary Capture Image Storage",
+    "1.2.840.10008.5.1.4.1.1.7.3": "Multi-frame Grayscale Word Secondary Capture Image Storage",
+    "1.2.840.10008.5.1.4.1.1.7.4": "Multi-frame True Color Secondary Capture Image Storage",
+    "1.2.840.10008.5.1.4.1.1.12.1": "X-Ray Angiographic Image Storage",
+    "1.2.840.10008.5.1.4.1.1.12.1.1": "Enhanced XA Image Storage",
+    "1.2.840.10008.5.1.4.1.1.12.2": "X-Ray Radiofluoroscopic Image Storage",
+    "1.2.840.10008.5.1.4.1.1.12.2.1": "Enhanced XRF Image Storage",
+    "1.2.840.10008.5.1.4.1.1.13.1.1": "X-Ray 3D Angiographic Image Storage",
+    "1.2.840.10008.5.1.4.1.1.13.1.2": "X-Ray 3D Craniofacial Image Storage",
+    "1.2.840.10008.5.1.4.1.1.13.1.3": "Breast Tomosynthesis Image Storage",
+    "1.2.840.10008.5.1.4.1.1.20": "Nuclear Medicine Image Storage",
+    "1.2.840.10008.5.1.4.1.1.77.1.1": "VL Endoscopic Image Storage",
+    "1.2.840.10008.5.1.4.1.1.77.1.2": "VL Microscopic Image Storage",
+    "1.2.840.10008.5.1.4.1.1.77.1.3": "VL Slide-Coordinates Microscopic Image Storage",
+    "1.2.840.10008.5.1.4.1.1.77.1.4": "VL Photographic Image Storage",
+    "1.2.840.10008.5.1.4.1.1.128": "Positron Emission Tomography Image Storage",
+    "1.2.840.10008.5.1.4.1.1.128.1": "Legacy Converted Enhanced PET Image Storage",
+    "1.2.840.10008.5.1.4.1.1.130": "Enhanced PET Image Storage",
+    "1.2.840.10008.5.1.4.1.1.481.1": "RT Image Storage",
+}
 
 
 class InvalidDicomError(Exception):
@@ -254,18 +299,19 @@ def read_header(path, head_bytes: int = 1 << 18) -> Dataset:
     return ds
 
 
-def read_frames(paths, out=None, threads: int = 8):
+def read_frames(paths, out=None, threads: int = 8, headers=None):
     """Batched ingest (the reference reads one file at a time: core/io.py:73-84 + core/image.py:1431-1444): parse the headers, then
     read every file's pixel bytes with ``readinto`` STRAIGHT into its slot of one [n, rows, cols] array -- pass a page-locked array
     (``_native.pinned_empty``) as `out` and the bytes go page cache -> pinned memory -> HBM with no intermediate copy.  All files
-    must share rows / columns / stored dtype.  Returns (frames, headers)."""
+    must share rows / columns / stored dtype.  `headers`: the files' ``read_header`` datasets when the caller already has them.
+    Returns (frames, headers)."""
     from concurrent.futures import ThreadPoolExecutor
 
     paths = [str(p) for p in paths]
     if not paths:
         raise ValueError("no files")
     with ThreadPoolExecutor(max(1, min(threads, len(paths)))) as pool:
-        headers = list(pool.map(read_header, paths))
+        headers = list(pool.map(read_header, paths)) if headers is None else list(headers)
         h0 = headers[0]
         shape = (int(h0["Rows"]), int(h0["Columns"]))
         dt = h0["PixelDtype"]

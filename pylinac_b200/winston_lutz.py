@@ -321,6 +321,39 @@ class WinstonLutz2D(ResultsDataMixin[WinstonLutz2DResult]):
                                    cax2epid_distance=r.cax2epid_distance, bb_location=ser(r.bb), field_cax=ser(r.field_cax))
 
 
+def cbct_frames(volume, ratio: float, *, device: int | None = None):
+    """The four frames WinstonLutz.from_cbct analyses (winston_lutz.py:1465-1505), on the device, from a CT volume [N, H, W] of
+    int16 / uint16 slices in sorted order and ratio = SliceThickness / PixelSpacing[0]: the maximum-intensity projections over rows
+    and columns (epid_stack_mip), their slice axis resampled by ``zoom(p, (1, ratio), grid_mode=True, mode='nearest', order=1)``
+    (epid_zoom on each projection row), then rot90 / fliplr, scipy's integer rounding and the uint16 bits array_to_dicom writes
+    (epid_cbct_views).  Returns [(uint16 device Batch, set indices)] in the order of the reference's file names G=0, G=180, G=270,
+    G=90 (top, bottom, left, right): one batch of 4 for square slices, else one per frame shape."""
+    ctx = nat.Context.default(device)
+    vol = nat.Batch.upload(ctx, volume)
+    try:
+        colmax, rowmax = nat.stack_mip(ctx, vol)
+    finally:
+        vol.free()
+    try:
+        zc = colmax._unary(nat.lib().epid_zoom, float(ratio), 1, 3)     # order 1, mode 'nearest' | grid_mode
+        try:
+            zr = rowmax._unary(nat.lib().epid_zoom, float(ratio), 1, 3)
+        except BaseException:
+            zc.free()
+            raise
+    finally:
+        colmax.free()
+        rowmax.free()
+    try:
+        src = np.asarray(volume).dtype
+        if zc.shape_dtype[0] == zr.shape_dtype[0]:
+            return [(nat.cbct_views(ctx, zr, zc, src), [0, 1, 2, 3])]
+        return [(nat.cbct_views(ctx, zr, None, src), [0, 1]), (nat.cbct_views(ctx, zc, None, src), [2, 3])]
+    finally:
+        zc.free()
+        zr.free()
+
+
 # ---------------------------------------------------------------------------------------------------------------- set level
 class MachineScale(enum.Enum):
     """core/scale.py:30-72 (axis conversions relative to IEC 61217)."""
@@ -482,7 +515,10 @@ class WinstonLutz(ResultsDataMixin[WinstonLutzResult]):
     host work on N result rows, as in the reference.
 
     ``WinstonLutz(directory_or_paths)`` loads DICOM files like the reference; ``WinstonLutz.from_arrays(frames, axes, dpmm=)``
-    takes frames already in memory (uint16 [n,h,w]) with one (gantry, collimator, couch) triple per frame."""
+    takes frames already in memory (uint16 [n,h,w]) with one (gantry, collimator, couch) triple per frame;
+    ``WinstonLutz.from_cbct(directory)`` builds four frames from a CBCT series on the device."""
+
+    is_from_cbct: bool = False
 
     def __init__(self, directory, use_filenames: bool = False, axis_mapping: dict | None = None, axes_precision: int | None = None,
                  dpi: float | None = None, sid: float | None = None, missing_axis_value=0):
@@ -518,12 +554,65 @@ class WinstonLutz(ResultsDataMixin[WinstonLutzResult]):
         self._setup(np.asarray(frames), [tuple(float(v) for v in a) for a in axes], float(dpmm))
         return self
 
+    @classmethod
+    def from_cbct_zip(cls, file, raw_pixels: bool = False, **kwargs):
+        """winston_lutz.py:1426-1442: ``from_cbct`` on the contents of a ZIP archive."""
+        with image.TemporaryZipDirectory(file) as tmp:
+            return cls.from_cbct(tmp, raw_pixels=raw_pixels, **kwargs)
+
+    @classmethod
+    def from_cbct(cls, directory, raw_pixels: bool = False, **kwargs):
+        """winston_lutz.py:1444-1509: a 4-angle Winston-Lutz set from a CBCT series.  The two maximum-intensity projections of the
+        volume, their slice axis resampled to square pixels, are "viewed" from the left, top, right and bottom as gantry 270 / 0 / 90
+        / 180 images; ``analyze()`` then forces ``low_density_bb`` and ``open_field``.  The volume goes to the GPU once
+        (epid_stack_mip, epid_zoom, epid_cbct_views) and the four frames stay there for the analysis; no file is written.
+
+        ``kwargs`` are WinstonLutz's (``use_filenames``, ``axis_mapping``, ``axes_precision``, ``missing_axis_value``; ``dpi`` / ``sid``
+        are accepted as there) and resolve the axes of the images the reference writes: files ``G=270``, ``G=0``, ``G=90``,
+        ``G=180`` with those gantry angles, collimator and couch 0.  Only integer frames are analysed: with ``raw_pixels=False`` a
+        series whose rescale tags turn the slices into float Hounsfield units raises NotImplementedError; pass ``raw_pixels=True``
+        (as the reference's docstring advises)."""
+        stack = image.DicomImageStack(directory, min_number=10, raw_pixels=raw_pixels)
+        return cls._from_stack(stack, **kwargs)
+
+    @classmethod
+    def _from_stack(cls, stack, use_filenames: bool = False, axis_mapping: dict | None = None, axes_precision: int | None = None,
+                    dpi: float | None = None, sid: float | None = None, missing_axis_value=0):
+        if any(im.array.dtype.kind == "f" or not np.may_share_memory(im.array, stack.volume) for im in stack.images):
+            raise NotImplementedError("WinstonLutz.from_cbct analyses the stored integer slices only; this series' rescale turns them "
+                                      "into other values. Pass raw_pixels=True.")
+        md = stack.metadata
+        pixel_mm = md.PixelSpacing[0]
+        file_dpi = 25.4 / pixel_mm
+        # array_to_dicom writes ImagePlanePixelSpacing = 25.4 / dpi, RTImageSID 1000 and RadiationMachineSAD 1000.0 (array_utils.py:281-283)
+        dpmm = (1 / (25.4 / file_dpi)) * (1000 / 1000.0)
+        names = sorted(f"G={g}" for g in (270, 0, 90, 180))       # the reference's file names, in this class's directory order
+        axes = []
+        for name in names:
+            if axis_mapping and not use_filenames and name in axis_mapping:
+                axes.append(tuple(float(v) for v in axis_mapping[name]))
+                continue
+            tags = {"gantry": float(f"{float(name[2:]):.2f}"), "coll": float(f"{0:.2f}"), "couch": float(f"{0:.2f}")}
+            axes.append(tuple(image.linac_axis_value(key, None, name, tags[key], use_filenames=use_filenames,
+                                                     missing_axis_value=missing_axis_value, axes_precision=axes_precision)
+                              for key in ("gantry", "coll", "couch")))
+        groups = cbct_frames(stack.volume, md.SliceThickness / pixel_mm)
+        self = cls.__new__(cls)
+        self._setup_groups(groups, axes, dpmm)
+        self.is_from_cbct = True
+        return self
+
     def _setup(self, frames: np.ndarray, axes, dpmm: float):
         if frames.ndim != 3 or len(axes) != frames.shape[0]:
             raise ValueError("frames must be [n,h,w] with one (gantry, collimator, couch) triple per frame")
         if frames.dtype != np.uint16:
             frames = image.frame_u16(frames, "GPU Winston-Lutz")
-        self._frames, self._axes, self.dpmm = frames, axes, dpmm
+        self._setup_groups([(frames, list(range(len(axes))))], axes, dpmm)
+        self._frames = frames
+
+    def _setup_groups(self, groups, axes, dpmm: float):
+        """groups: (uint16 frames [k,h,w] ndarray or device Batch, the set indices of those k images); one batch per frame shape"""
+        self._groups, self._axes, self.dpmm = groups, axes, dpmm
         self.images: list[_SetImage] = []
         self._is_analyzed = False
         self.machine_scale = MachineScale.IEC61217
@@ -535,8 +624,15 @@ class WinstonLutz(ResultsDataMixin[WinstonLutzResult]):
                 collimator_reference: float = 0, couch_reference: float = 0, bb_proximity_mm: float = 20) -> None:
         """winston_lutz.py:1519-1611"""
         self.machine_scale = machine_scale
-        rows = analyze_batch(self._frames, self.dpmm, bb_size_mm=bb_size_mm, low_density_bb=low_density_bb, open_field=open_field,
-                             bb_proximity_mm=bb_proximity_mm)
+        if self.is_from_cbct:      # winston_lutz.py:1564-1566
+            low_density_bb = True
+            open_field = True
+        rows = [None] * len(self._axes)
+        for frames, idx in self._groups:
+            res = analyze_batch(frames, self.dpmm, bb_size_mm=bb_size_mm, low_density_bb=low_density_bb, open_field=open_field,
+                                bb_proximity_mm=bb_proximity_mm)
+            for j, k in enumerate(idx):
+                rows[k] = res[j]
         refs = dict(snap_tolerance=snap_tolerance, gantry_reference=gantry_reference, collimator_reference=collimator_reference,
                     couch_reference=couch_reference)
         self.images = []
