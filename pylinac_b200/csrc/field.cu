@@ -19,7 +19,8 @@
 // lets it (tests/test_oracle_field.py), so the top_* fields are outside the parity bar.
 //
 // Stages:
-//   k_frame_stats    exact p5 / p50 / p95 + min / max + exact row and column sums of every frame            (stats.cu)
+//   k_inv_* / k_hist_view  min / max + exact row and column sums of every frame; the p5 / p50 / p95 inversion decision,
+//                    certified from exact counts or read from the exact histogram                                  (stats.cu)
 //   k_field_center   CTA per (frame, axis): inversion decision, SingleProfile(sum profile).beam_center() -> strip position
 //   k_field_strips   CTA per (frame, axis): mean over the strip of rows / columns -> raw profile
 //   k_field_profile  CTA per (frame, axis): SingleProfile(profile, dpmm, ...) -> penumbra, centres, field sizes, slopes,
@@ -970,18 +971,6 @@ k_single_profile(const epid_sp_params p, const double* __restrict__ raw, const d
 
 using namespace epid;
 
-namespace {
-
-__global__ void k_field_refs(const uint16_t* base, int n, int H, int W, FrameRef* refs) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    refs[i].origin = base + (size_t)i * H * W;
-    refs[i].pitch = W;
-    refs[i].pad = 0;
-}
-
-}  // namespace
-
 extern "C" int32_t epid_field_profile_len(int32_t n0, double dpmm, int32_t interpolation, double resolution_mm) {
     if (!interpolation) return n0;
     return (int32_t)rint((double)n0 / (dpmm * resolution_mm));
@@ -1047,8 +1036,7 @@ extern "C" int32_t epid_field_analyze(epid_ctx* ctx, const epid_batch* frames, c
         EPID_CUDA(cudaMemcpyAsync(d_gv, gauss_v, sizeof(double) * (size_t)(2 * lw_v + 1), cudaMemcpyHostToDevice, st));
     }
     EPID_CUDA(cudaMemsetAsync(d_res, 0, sizeof(epid_field_result) * n, st));
-    k_field_refs<<<(n + 127) / 128, 128, 0, st>>>((const uint16_t*)frames->dptr, n, H, W, d_rf);
-    ctx->launches++;
+    launch_refs_from_batch(ctx, st, (const uint16_t*)frames->dptr, n, H, W, 0, 0, d_rf);
     StatsGeom g;
     rc = make_stats_geom(&g, H, W);
     if (rc != EPID_OK) return rc;

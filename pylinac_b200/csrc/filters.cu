@@ -203,14 +203,6 @@ static int run_median_generic(epid_ctx* ctx, const epid_batch* in, epid_batch* o
     return EPID_OK;
 }
 
-__global__ void k_refs_compact(const uint16_t* base, int n, int H, int W, FrameRef* refs) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    refs[i].origin = base + (size_t)i * H * W;
-    refs[i].pitch = W;
-    refs[i].pad = 0;
-}
-
 static int sync_and_check(epid_ctx* ctx, int rc, epid_batch** out) {
     if (rc == EPID_OK) {
         cudaError_t e = cudaStreamSynchronize(ctx->stream);
@@ -263,9 +255,8 @@ int32_t epid_median_filter(epid_ctx* ctx, const epid_batch* in, int32_t size, ep
         if (rc == EPID_OK) {
             FrameRef* src = (FrameRef*)ctx->scratch;
             FrameRef* dst = (FrameRef*)((char*)ctx->scratch + (sizeof(FrameRef) * n + 255) / 256 * 256);
-            k_refs_compact<<<(n + 127) / 128, 128, 0, ctx->stream>>>((const uint16_t*)in->dptr, n, in->h, in->w, src);
-            k_refs_compact<<<(n + 127) / 128, 128, 0, ctx->stream>>>((const uint16_t*)(*out)->dptr, n, in->h, in->w, dst);
-            ctx->launches += 2;
+            launch_refs_from_batch(ctx, ctx->stream, (const uint16_t*)in->dptr, n, in->h, in->w, 0, 0, src);
+            launch_refs_from_batch(ctx, ctx->stream, (const uint16_t*)(*out)->dptr, n, in->h, in->w, 0, 0, dst);
             rc = launch_median_u16(ctx, ctx->stream, src, dst, nullptr, nullptr, n, in->h, in->w, size);
         }
     } else {

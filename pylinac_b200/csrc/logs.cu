@@ -261,8 +261,7 @@ __global__ void k_inv_apply(const double* __restrict__ in, double* __restrict__ 
     double v[SEL_RANKS];
 #pragma unroll
     for (int r = 0; r < SEL_RANKS; r++) v[r] = okey_value(st[f].prefix[r]);
-    auto lerp = [](double a, double b, double t) { const double d = b - a; double r = a + d * t; if (t >= 0.5) r = b - d * (1.0 - t); return r; };
-    const double p_low = lerp(v[2], v[3], p.g_low), p_mid = lerp(v[4], v[5], p.g_mid), p_high = lerp(v[6], v[7], p.g_high);
+    const double p_low = np_lerp(v[2], v[3], p.g_low), p_mid = np_lerp(v[4], v[5], p.g_mid), p_high = np_lerp(v[6], v[7], p.g_high);
     const bool inv = fabs(p_mid - p_low) > fabs(p_mid - p_high);
     if (blockIdx.x == 0 && threadIdx.x == 0 && inverted) inverted[f] = inv ? 1 : 0;
     const double mn = v[0], mx = v[1];

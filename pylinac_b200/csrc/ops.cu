@@ -229,25 +229,8 @@ static int finish(epid_ctx* ctx, int rc, epid_batch** out) {
 }
 
 // ---------------------------------------------------------------------------------------- statistics API helpers
-__global__ void k_refs_from_batch(const uint16_t* base, int n, int H0, int W0, int r0, int c0, FrameRef* refs) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    refs[i].origin = base + (size_t)i * H0 * W0 + (size_t)r0 * W0 + c0;
-    refs[i].pitch = W0;
-    refs[i].pad = 0;
-}
-
 __global__ void k_u8_to_u16(const uint8_t* __restrict__ in, uint16_t* __restrict__ out, size_t total) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) out[i] = in[i];
-}
-
-__global__ void k_hist_global(const FrameRef* __restrict__ refs, int H, int W, uint32_t* __restrict__ hist) {
-    const FrameRef r = refs[blockIdx.y];
-    uint32_t* h = hist + (size_t)blockIdx.y * 65536;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < H * W; i += gridDim.x * blockDim.x) {
-        const int y = i / W, x = i - y * W;
-        atomicAdd(h + __ldg(r.origin + (size_t)y * r.pitch + x), 1u);
-    }
 }
 
 }  // namespace epid
@@ -371,9 +354,8 @@ int32_t epid_frame_stats(epid_ctx* ctx, const epid_batch* b, int32_t r0, int32_t
     FrameStats* st = (FrameStats*)p; p += (sizeof(FrameStats) * n + 255) / 256 * 256;
     uint32_t* d_row = (uint32_t*)p; p += (sizeof(uint32_t) * (size_t)n * vh + 255) / 256 * 256;
     uint32_t* d_col = (uint32_t*)p;
-    k_refs_from_batch<<<(n + 127) / 128, 128, 0, ctx->stream>>>(base, n, b->h, b->w, r0, c0, refs);
-    ctx->launches++;
-    rc = launch_frame_stats(ctx, ctx->stream, g, refs, nullptr, n, st, d_row, d_col);
+    launch_refs_from_batch(ctx, ctx->stream, base, n, b->h, b->w, r0, c0, refs);
+    rc = launch_frame_stats(ctx, ctx->stream, g, refs, n, st, d_row, d_col);
     std::vector<FrameStats> hs(n);
     std::vector<uint32_t> hrow, hcol;
     if (rc == EPID_OK) {
@@ -389,14 +371,7 @@ int32_t epid_frame_stats(epid_ctx* ctx, const epid_batch* b, int32_t r0, int32_t
         if (mn) mn[i] = hs[i].mn;
         if (mx) mx[i] = hs[i].mx;
         if (sum) sum[i] = (double)hs[i].sum;
-        for (int k = 0; k < nq && pct; k++) {
-            // numpy _lerp
-            const double a = hs[i].ostat[2 * k], bb = hs[i].ostat[2 * k + 1], t = gam[k];
-            const double d = bb - a;
-            double r = a + d * t;
-            if (t >= 0.5) r = bb - d * (1.0 - t);
-            pct[(size_t)i * nq + k] = r;
-        }
+        for (int k = 0; k < nq && pct; k++) pct[(size_t)i * nq + k] = np_lerp(hs[i].ostat[2 * k], hs[i].ostat[2 * k + 1], gam[k]);
     }
     if (rowsum) for (size_t i = 0; i < hrow.size(); i++) rowsum[i] = hrow[i];
     if (colsum) for (size_t i = 0; i < hcol.size(); i++) colsum[i] = hcol[i];
@@ -416,10 +391,14 @@ int32_t epid_frame_histogram(epid_ctx* ctx, const epid_batch* b, int32_t r0, int
     if (rc != EPID_OK) { if (tmp) cudaFree(tmp); return rc; }
     FrameRef* refs = (FrameRef*)ctx->scratch;
     uint32_t* d_hist = (uint32_t*)((char*)ctx->scratch + (sizeof(FrameRef) * n + 255) / 256 * 256);
-    k_refs_from_batch<<<(n + 127) / 128, 128, 0, ctx->stream>>>(base, n, b->h, b->w, r0, c0, refs);
-    cudaMemsetAsync(d_hist, 0, sizeof(uint32_t) * (size_t)n * 65536, ctx->stream);
-    k_hist_global<<<dim3(64, n), 256, 0, ctx->stream>>>(refs, vh, vw, d_hist);
-    ctx->launches += 2;
+    launch_refs_from_batch(ctx, ctx->stream, base, n, b->h, b->w, r0, c0, refs);
+    // any view width: the geometry is not limited to STATS_MAX_DIM like make_stats_geom's
+    StatsGeom g;
+    memset(&g, 0, sizeof(g));
+    g.H = vh;
+    g.W = vw;
+    rc = launch_frame_histogram(ctx, ctx->stream, g, refs, n, d_hist);
+    if (rc != EPID_OK) { if (tmp) cudaFree(tmp); return rc; }
     cudaError_t e = cudaMemcpyAsync(hist, d_hist, sizeof(uint32_t) * (size_t)n * 65536, cudaMemcpyDeviceToHost, ctx->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
     if (tmp) cudaFree(tmp);

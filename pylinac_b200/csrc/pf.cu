@@ -14,7 +14,8 @@
 // in fp64 (same operation order as numpy/scipy, FMA contraction disabled).
 //
 // Stages (all stream-ordered, no host round trip unless a frame is flagged noisy):
-//   k_frame_stats   1 read   min/max/sum/row+col sums/corner boxes/exact p0.5,p99.5,median   (stats.cu)
+//   k_hist_view     1 read   exact histogram, row sums, column partials                       (stats.cu)
+//   k_stats_from_hist -      min/max/sum/col sums/corner boxes/exact p0.5,p99.5,median         (stats.cu)
 //   k_pf_decide     -        noise flag, corner inversion, D, median in g units
 //   k_pf_clamp_sums 1 read   row/col sums of max(2g, 2*median)  (orientation; skipped if orientation is given)
 //   k_pf_profile    -        orientation, leaf profile, find_peaks -> pickets, spacing, leaves in view
@@ -70,7 +71,8 @@ __global__ void k_pf_decide(const PfConst* __restrict__ cc, const FrameStats* __
 
 // ------------------------------------------------------------------------------------------------ clamped sums
 // PicketFence.orientation (picketfence.py:1509-1514): temp[temp < median] = median; np.sum(temp, 0); np.sum(temp, 1).
-// In 2g units: sum of max(2g, med2).  Same CTA-per-frame streaming structure as k_frame_stats.
+// In 2g units: sum of max(2g, med2).  One persistent CTA per SM streams a frame at a time: each thread owns a fixed 8-pixel column
+// vector and strides over rows (StatsGeom vprp / groups).
 __global__ void __launch_bounds__(STATS_THREADS, 1)
 k_pf_clamp_sums(const StatsGeom g, const FrameRef* __restrict__ frames, const PfFrame* __restrict__ fr, int nframes,
                 uint32_t* __restrict__ rowsum2, uint32_t* __restrict__ colsum2) {
@@ -470,14 +472,6 @@ __global__ void k_pf_swap_refs(FrameRef* refs, const FrameRef* refs_b, const int
     if (select[i]) refs[i] = refs_b[i];
 }
 
-__global__ void k_pf_set_dst_refs(FrameRef* refs_b, uint16_t* pool, int n, int H, int Wp) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    refs_b[i].origin = pool + (size_t)i * H * Wp;
-    refs_b[i].pitch = Wp;
-    refs_b[i].pad = 0;
-}
-
 // Enqueue the whole pipeline for one device-resident batch on `stream`; results land in w.summ / w.meas (device).
 // pf_front.cu
 bool pf_front_supported(int H, int W, int pitch);
@@ -617,15 +611,15 @@ static int pf_run(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, 
     const int tb = 128, nb = (n + tb - 1) / tb;
     k_pf_init<<<nb, tb, 0, stream>>>(d_frames, n, H0, W0, crop, w.refs, w.fr, w.counters, d_sel);
     ctx->launches++;
-    // bench timers: around the frame-streaming kernel only (k_pf_stream inside launch_pf_front, k_frame_stats otherwise)
+    // bench timers: around the frame-streaming kernel only (k_pf_stream inside launch_pf_front, the exact frame statistics otherwise)
     if (fast) {
         if (redo) {      // certify _has_noise() == True by one exact count, filter those frames into the pool (see k_pf_count_above)
             const int Wp = (W + 7) / 8 * 8;
             EPID_CUDA(cudaMemsetAsync(w.sel_idx, 0, sizeof(int) * n, stream));
             k_pf_count_above<<<dim3(CA_PARTS, n), 256, 0, stream>>>(w.refs, redo->raw_fr, d_sel, H, W, w.sel_idx);
             k_pf_mark_certified<<<nb, tb, 0, stream>>>(w.sel_idx, n, npix - 1 - (int)hc.hi.next, w.select);
-            k_pf_set_dst_refs<<<nb, tb, 0, stream>>>(w.refs_b, redo->pool, n, H, Wp);
-            ctx->launches += 3;
+            ctx->launches += 2;
+            launch_refs_from_batch(ctx, stream, redo->pool, n, H, Wp, 0, 0, w.refs_b);
             rc = launch_median_u16(ctx, stream, w.refs, w.refs_b, nullptr, w.select, n, H, W, 3);
             if (rc != EPID_OK) return rc;
             k_pf_swap_refs<<<nb, tb, 0, stream>>>(w.refs, w.refs_b, w.select, n);
@@ -640,7 +634,7 @@ static int pf_run(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, 
         if (front_evt) EPID_CUDA(cudaEventRecord(front_evt, stream));
     } else {
         if (tm && tm->on) { rc = tm->record(stream); if (rc != EPID_OK) return rc; }
-        rc = launch_frame_stats(ctx, stream, g, w.refs, nullptr, n, w.stats, w.rowsum, w.colsum);
+        rc = launch_frame_stats(ctx, stream, g, w.refs, n, w.stats, w.rowsum, w.colsum);
         if (rc == EPID_OK && tm && tm->on) rc = tm->record(stream);
     }
     if (rc != EPID_OK) return rc;
@@ -668,8 +662,8 @@ static int pf_run(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, 
         rc = ensure_pool(cur_pool);
         if (rc != EPID_OK) return rc;
         k_pf_mark_noisy<<<nb, tb, 0, stream>>>(w.fr, n, w.select, w.maps);
-        k_pf_set_dst_refs<<<nb, tb, 0, stream>>>(w.refs_b, pools[cur_pool], n, H, Wp);
-        ctx->launches += 2;
+        ctx->launches++;
+        launch_refs_from_batch(ctx, stream, pools[cur_pool], n, H, Wp, 0, 0, w.refs_b);
         rc = launch_median_u16(ctx, stream, w.refs, w.refs_b, nullptr, w.select, n, H, W, 3);
         if (rc != EPID_OK) return rc;
         k_pf_swap_refs<<<nb, tb, 0, stream>>>(w.refs, w.refs_b, w.select, n);
@@ -678,7 +672,7 @@ static int pf_run(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, 
         // would recompute identical numbers, so run it on all frames -- flagged ones are rare and this keeps
         // one code path.
         EPID_CUDA(cudaMemsetAsync(w.counters, 0, sizeof(int), stream));
-        rc = launch_frame_stats(ctx, stream, g, w.refs, nullptr, n, w.stats, w.rowsum, w.colsum);
+        rc = launch_frame_stats(ctx, stream, g, w.refs, n, w.stats, w.rowsum, w.colsum);
         if (rc != EPID_OK) return rc;
         k_pf_decide<<<nb, tb, 0, stream>>>(w.cst, w.stats, w.fr, n, w.select, 1, w.counters);
         ctx->launches++;
@@ -692,8 +686,8 @@ static int pf_run(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, 
         rc = ensure_pool(2);
         if (rc != EPID_OK) return rc;
         k_pf_prepare_filter<<<nb, tb, 0, stream>>>(w.fr, n, w.select, w.maps, p->invert);
-        k_pf_set_dst_refs<<<nb, tb, 0, stream>>>(w.refs_b, pools[2], n, H, Wp);
-        ctx->launches += 2;
+        ctx->launches++;
+        launch_refs_from_batch(ctx, stream, pools[2], n, H, Wp, 0, 0, w.refs_b);
         rc = launch_median_u16(ctx, stream, w.refs, w.refs_b, w.maps, w.select, n, H, W, p->filter_size);
         if (rc != EPID_OK) return rc;
         k_pf_swap_refs<<<nb, tb, 0, stream>>>(w.refs, w.refs_b, w.select, n);
@@ -702,7 +696,7 @@ static int pf_run(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, 
         EPID_CUDA(cudaMemcpyAsync(w.cst, &hc, sizeof(hc), cudaMemcpyHostToDevice, stream));
         StatsGeom g2 = g;
         g2.box = 0;
-        rc = launch_frame_stats(ctx, stream, g2, w.refs, nullptr, n, w.stats, w.rowsum, w.colsum);
+        rc = launch_frame_stats(ctx, stream, g2, w.refs, n, w.stats, w.rowsum, w.colsum);
         if (rc != EPID_OK) return rc;
         k_pf_decide<<<nb, tb, 0, stream>>>(w.cst, w.stats, w.fr, n, nullptr, 0, w.counters);
         ctx->launches++;

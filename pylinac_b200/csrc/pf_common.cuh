@@ -68,14 +68,6 @@ struct alignas(16) PfWinRec {              // one per window, 400 bytes
 };
 static_assert(sizeof(PfWinRec) == 400, "PfWinRec layout");
 
-// numpy _lerp (numpy/lib/_function_base_impl.py): a + (b-a)*t, and b - (b-a)*(1-t) where t >= 0.5
-__device__ __forceinline__ double np_lerp(double a, double b, double t) {
-    const double d = b - a;
-    double r = a + d * t;
-    if (t >= 0.5) r = b - d * (1.0 - t);
-    return r;
-}
-
 // noise flag (_has_noise), corner inversion, D, median in g units for one frame from its statistics.
 // check_noise: evaluate the noise criterion (and count noisy frames in counters[0]); post_filter: statistics were taken
 // on an already inverted + filtered copy, only D / median are refreshed.

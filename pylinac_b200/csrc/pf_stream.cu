@@ -643,7 +643,7 @@ k_pf_tail(const PfConst* __restrict__ cc, const StatsGeom g, const StreamGeom sg
             f.med2 = f.inv ? 2u * (mx - min(po.a1, mx)) : 2u * (max(po.a1, mn) - mn);
         }
         FrameStats st;
-        st.mn = mn; st.mx = mx; st.npix = npix; st.overflow = bad ? 1u : 0u;
+        st.mn = mn; st.mx = mx; st.npix = npix; st.inv_certified = 0;
         st.sum = s_sum; st.corner_sum = s_corner;
         for (int i = 0; i < STATS_MAX_RANKS; i++) st.ostat[i] = 0;
         st.ostat[0] = mn; st.ostat[1] = po.u_lo; st.ostat[2] = po.l_hi; st.ostat[3] = mx; st.ostat[4] = po.a1; st.ostat[5] = po.b1;

@@ -19,7 +19,8 @@
 // (FMA contraction disabled), so peak indices are bit-exact and the wobble agrees to ~1e-12 px.
 //
 // Stages:
-//   k_frame_stats    exact order statistics of the frame (p4 / p50 / p96) and of its central third (p90)      (stats.cu)
+//   k_inv_* / k_hist_view  the frame's p4 / p50 / p96 inversion decision (certified from exact counts or read from the exact
+//                    histogram); exact p90 of its central third from the exact histogram                           (stats.cu)
 //   k_star_front     inversion decision, central-third column / row maxima, FW80M start point, local maximum
 //   k_star_rows      CTA per (frame, candidate row): ring sampling (20 radii, nearest neighbour) -> roll -> gaussian -> ground once per
 //                    radius, then per min_peak_height: find_fwxm_peaks -> lines -> Nelder-Mead until a candidate has a verdict
@@ -652,21 +653,6 @@ k_circle_profile(const T* __restrict__ img, int H, int W, double cx, double cy, 
 
 using namespace epid;
 
-namespace {
-
-__global__ void k_star_refs(const uint16_t* base, int n, int H, int W, int top, int left, FrameRef* full, FrameRef* central) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    full[i].origin = base + (size_t)i * H * W;
-    full[i].pitch = W;
-    full[i].pad = 0;
-    central[i].origin = base + (size_t)i * H * W + (size_t)top * W + left;
-    central[i].pitch = W;
-    central[i].pad = 0;
-}
-
-}  // namespace
-
 extern "C" int32_t epid_starshot_analyze(epid_ctx* ctx, const epid_batch* frames, const epid_star_params* p, const double* gauss_weights,
                                          const int32_t* gauss_offsets, int32_t max_sigma, epid_star_result* results) {
     EPID_REQUIRE(ctx && frames && p && gauss_weights && gauss_offsets && results, EPID_ERR_INVALID, "NULL argument");
@@ -722,8 +708,8 @@ extern "C" int32_t epid_starshot_analyze(epid_ctx* ctx, const epid_batch* frames
     EPID_CUDA(cudaMemcpyAsync(d_gw, gauss_weights, sizeof(double) * gw_count, cudaMemcpyHostToDevice, st));
     EPID_CUDA(cudaMemcpyAsync(d_go, gauss_offsets, sizeof(int) * (max_sigma + 1), cudaMemcpyHostToDevice, st));
     EPID_CUDA(cudaMemsetAsync(d_res, 0, sizeof(epid_star_result) * n, st));
-    k_star_refs<<<(n + 127) / 128, 128, 0, st>>>((const uint16_t*)frames->dptr, n, H, W, hc.top, hc.left, d_rf, d_rc);
-    ctx->launches++;
+    launch_refs_from_batch(ctx, st, (const uint16_t*)frames->dptr, n, H, W, 0, 0, d_rf);
+    launch_refs_from_batch(ctx, st, (const uint16_t*)frames->dptr, n, H, W, hc.top, hc.left, d_rc);
     // exact order statistics: frame (p4, p50, p96) and central third (p90 and its mirror for flipped frames)
     StatsGeom g;
     rc = make_stats_geom(&g, H, W);
@@ -743,7 +729,7 @@ extern "C" int32_t epid_starshot_analyze(epid_ctx* ctx, const epid_batch* frames
     gc.ranks[0] = hc.p90.prev; gc.ranks[1] = hc.p90.next;
     gc.ranks[2] = nc - 1 - hc.p90.next; gc.ranks[3] = nc - 1 - hc.p90.prev;
     gc.box = 0;
-    rc = launch_frame_stats(ctx, st, gc, d_rc, nullptr, n, d_sc, nullptr, nullptr);
+    rc = launch_frame_stats(ctx, st, gc, d_rc, n, d_sc, nullptr, nullptr);
     if (rc != EPID_OK) return rc;
     {
         const int n_max = hc.cw > hc.ch ? hc.cw : hc.ch;

@@ -1,24 +1,12 @@
-// Fused frame statistics: ONE streaming read of a uint16 frame view produces min, max, sum, row sums,
-// column sums, the four check_inversion corner sums and EXACT order statistics (from a 65536-bin histogram
-// that never leaves shared memory).
+// Frame statistics of uint16 frame views: min, max, sum, row sums, column sums, the four check_inversion corner sums and EXACT order
+// statistics from a 65536-bin histogram.
 //
 // Replaces the reference's numpy passes: array.min()/max() (picketfence.py:231-232, core/image.py:851),
 // np.percentile / np.median of the full frame (picketfence.py:233,1510; core/image.py:918-920),
 // np.mean(image, axis) (picketfence.py:748-750), corner means (core/image.py:881-896).
-//
-// Design: one persistent CTA of 1024 threads per SM, one frame per CTA at a time.  Each thread owns a
-// fixed 8-pixel column vector (128-bit ld.global.nc.L1::no_allocate, row pitch keeps it 16-byte aligned) and
-// strides over rows, so column sums live in registers, row sums are one warp-shuffle reduction + one shared
-// atomic per warp-row, and the histogram is 65536 packed 16-bit counters = 128 KB of shared memory updated
-// with ATOMS.ADD (1 or 0x10000 into the 32-bit word).  A packed counter can overflow only if > 65535 pixels of
-// a frame share one value; that is detected exactly (the decoded bin total then differs from the pixel count)
-// and the frame is re-run by the MODE 1 variant (32-bit counters over value>>1 plus a second pass resolving
-// the low bit), so results are always exact.
 #include "stats.cuh"
 
 namespace epid {
-
-constexpr int HIST_WORDS = 32768;
 
 int make_stats_geom(StatsGeom* g, int H, int W) {
     if (H <= 0 || W <= 0 || H > STATS_MAX_DIM || W > STATS_MAX_DIM) {
@@ -38,304 +26,51 @@ int make_stats_geom(StatsGeom* g, int H, int W) {
     return EPID_OK;
 }
 
-__device__ __forceinline__ void block_scan_excl_1024(uint32_t v, uint32_t* s_warp, uint32_t& excl, uint32_t& total) {
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-    uint32_t inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        uint32_t t = __shfl_up_sync(0xffffffffu, inc, o);
-        if (lane >= o) inc += t;
-    }
-    if (lane == 31) s_warp[wid] = inc;
-    __syncthreads();
-    if (wid == 0) {
-        uint32_t w = s_warp[lane];
-        uint32_t winc = w;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            uint32_t t = __shfl_up_sync(0xffffffffu, winc, o);
-            if (lane >= o) winc += t;
-        }
-        s_warp[lane] = winc - w;       // exclusive warp offsets
-        if (lane == 31) s_warp[32] = winc;
-    }
-    __syncthreads();
-    excl = s_warp[wid] + inc - v;
-    total = s_warp[32];
-    __syncthreads();
+__global__ void k_refs_from_batch(const uint16_t* base, int n, int H0, int W0, int r0, int c0, FrameRef* refs) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    refs[i].origin = base + (size_t)i * H0 * W0 + (size_t)r0 * W0 + c0;
+    refs[i].pitch = W0;
+    refs[i].pad = 0;
 }
 
-// MODE 0: packed u16 counters, all 65536 bins.  MODE 1: u32 counters over (v >> 1), low bit resolved by a 2nd pass.
-template <int MODE>
-__global__ void __launch_bounds__(STATS_THREADS, 1)
-k_frame_stats(const StatsGeom g, const FrameRef* __restrict__ frames, const int* __restrict__ out_index, int nframes,
-              FrameStats* __restrict__ stats, uint32_t* __restrict__ rowsum_out, uint32_t* __restrict__ colsum_out) {
-    extern __shared__ uint32_t smem[];
-    uint32_t* hist = smem;                                   // HIST_WORDS
-    uint32_t* colpart = hist + HIST_WORDS;                   // STATS_THREADS * 8
-    uint32_t* s_warp = colpart + STATS_THREADS * 8;          // 40
-    uint32_t* s_misc = s_warp + 40;                          // 8 + 3*STATS_MAX_RANKS (even word index: 64-bit atomics)
-    uint32_t* rowsum_sm = s_misc + 8 + 3 * STATS_MAX_RANKS;  // H
-
-    const int tid = threadIdx.x;
-    const int lane = tid & 31;
-    const int grp = tid / g.vprp;
-    const int jc = tid - grp * g.vprp;
-    const bool active_grp = grp < g.groups;
-
-    for (int fi = blockIdx.x; fi < nframes; fi += gridDim.x) {
-        const int slot = out_index ? out_index[fi] : fi;
-        if (MODE == 1 && stats[slot].overflow == 0) continue;
-        const FrameRef fr = frames[fi];
-        const uint16_t* __restrict__ f = fr.origin;
-        const int pitch = fr.pitch;
-        // aligned vector grid of this frame: vector j covers view columns [8j - mis, 8j - mis + 8)
-        const bool aligned = (pitch % 8) == 0;
-        const int mis = aligned ? (int)((reinterpret_cast<uintptr_t>(f) >> 1) & 7) : 0;
-        const int col_first = jc * 8 - mis;
-        uint32_t valid = 0;
-        if (active_grp) {
-#pragma unroll
-            for (int k = 0; k < 8; k++) {
-                const int c = col_first + k;
-                if (c >= 0 && c < g.W) valid |= 1u << k;
-            }
-        }
-        const bool active = valid != 0;
-        for (int i = tid; i < HIST_WORDS; i += STATS_THREADS) hist[i] = 0;
-        for (int i = tid; i < g.H; i += STATS_THREADS) rowsum_sm[i] = 0;
-        __syncthreads();
-
-        uint32_t mn = 0xffffu, mx = 0, csum[8];
-        unsigned long long tsum = 0;
-#pragma unroll
-        for (int k = 0; k < 8; k++) csum[k] = 0;
-
-        if (active_grp) {
-            constexpr int U = 4;
-            for (int r = grp; r < g.H; r += g.groups * U) {
-                uint4 q[U];
-#pragma unroll
-                for (int u = 0; u < U; u++) {
-                    const int rr = r + u * g.groups;
-                    q[u] = make_uint4(0, 0, 0, 0);
-                    if (rr < g.H && active) {
-                        const uint16_t* rowp = f + (size_t)rr * pitch;
-                        if (aligned) {
-                            q[u] = ldg_stream16(rowp + col_first);
-                        } else {
-                            uint32_t w[4] = {0, 0, 0, 0};
-#pragma unroll
-                            for (int k = 0; k < 8; k++)
-                                if (valid >> k & 1) w[k >> 1] |= (uint32_t)__ldg(rowp + col_first + k) << ((k & 1) * 16);
-                            q[u] = make_uint4(w[0], w[1], w[2], w[3]);
-                        }
-                    }
-                }
-#pragma unroll
-                for (int u = 0; u < U; u++) {
-                    const int rr = r + u * g.groups;
-                    if (rr >= g.H) break;  // warp-uniform
-                    uint32_t w[4] = {q[u].x, q[u].y, q[u].z, q[u].w};
-                    uint32_t rs = 0;
-                    if (valid == 0xffu) {
-#pragma unroll
-                        for (int k = 0; k < 4; k++) {
-                            const uint32_t lo = w[k] & 0xffffu, hi = w[k] >> 16;
-                            if (MODE == 0) {
-                                atomicAdd(&hist[lo >> 1], (lo & 1) ? 0x10000u : 1u);
-                                atomicAdd(&hist[hi >> 1], (hi & 1) ? 0x10000u : 1u);
-                            } else {
-                                atomicAdd(&hist[lo >> 1], 1u);
-                                atomicAdd(&hist[hi >> 1], 1u);
-                            }
-                            mn = min(mn, min(lo, hi));
-                            mx = max(mx, max(lo, hi));
-                            csum[2 * k] += lo;
-                            csum[2 * k + 1] += hi;
-                            rs += lo + hi;
-                        }
-                    } else if (valid) {
-#pragma unroll
-                        for (int k = 0; k < 8; k++) {
-                            if (valid >> k & 1) {
-                                const uint32_t v = (w[k >> 1] >> ((k & 1) * 16)) & 0xffffu;
-                                if (MODE == 0)
-                                    atomicAdd(&hist[v >> 1], (v & 1) ? 0x10000u : 1u);
-                                else
-                                    atomicAdd(&hist[v >> 1], 1u);
-                                mn = min(mn, v);
-                                mx = max(mx, v);
-                                csum[k] += v;
-                                rs += v;
-                            }
-                        }
-                    }
-                    tsum += rs;
-                    rs = warp_sum(rs);
-                    if (lane == 0) atomicAdd(&rowsum_sm[rr], rs);
-                }
-            }
-        }
-        // column partials -> shared
-#pragma unroll
-        for (int k = 0; k < 8; k++) colpart[tid * 8 + k] = active ? csum[k] : 0u;
-        // block reductions of min / max / sum
-        mn = warp_min(mn);
-        mx = warp_max(mx);
-        tsum = warp_sum(tsum);
-        __syncthreads();  // (also orders hist / rowsum / colpart writes)
-        if (tid == 0) { s_misc[0] = 0xffffu; s_misc[1] = 0; s_misc[2] = 0; s_misc[3] = 0; s_misc[4] = 0; s_misc[5] = 0; }
-        __syncthreads();
-        if (lane == 0) {
-            atomicMin(&s_misc[0], mn);
-            atomicMax(&s_misc[1], mx);
-            atomicAdd(reinterpret_cast<unsigned long long*>(&s_misc[2]), tsum);
-        }
-        // corner boxes (core/image.py:881-894): rows [rp, rp+box) and [H-rp-box, H-rp), cols [cp, cp+box) and [W-cp-box, W-cp)
-        if (g.box > 0) {
-            const int per = g.box * g.box;
-            unsigned long long cs = 0;
-            for (int i = tid; i < 4 * per; i += STATS_THREADS) {
-                const int b = i / per, o = i - b * per;
-                const int y = o / g.box, x = o - y * g.box;
-                const int rr = ((b & 2) ? g.H - g.rp - g.box : g.rp) + y;
-                const int cc = ((b & 1) ? g.W - g.cp - g.box : g.cp) + x;
-                if (rr >= 0 && rr < g.H && cc >= 0 && cc < g.W) cs += __ldg(f + (size_t)rr * pitch + cc);
-            }
-            cs = warp_sum(cs);
-            if (lane == 0 && cs) atomicAdd(reinterpret_cast<unsigned long long*>(&s_misc[4]), cs);
-        }
-        __syncthreads();
-        // outputs: sums
-        if (colsum_out) {
-            for (int x = tid; x < g.W; x += STATS_THREADS) {
-                const int ac = x + mis;  // position inside the per-row vector grid
-                uint32_t s = 0;
-                for (int gg = 0; gg < g.groups; gg++) s += colpart[(gg * g.vprp) * 8 + ac];
-                colsum_out[(size_t)slot * g.W + x] = s;
-            }
-        }
-        if (rowsum_out)
-            for (int y = tid; y < g.H; y += STATS_THREADS) rowsum_out[(size_t)slot * g.H + y] = rowsum_sm[y];
-
-        // ---- order statistics from the histogram
-        uint32_t cnt = 0;
-        {
-            const uint32_t* hw = hist + tid * 32;
-#pragma unroll 8
-            for (int i = 0; i < 32; i++) {
-                // rotate the start so that the 32 lanes of a warp hit 32 different banks
-                const uint32_t w = hw[(i + lane) & 31];
-                cnt += (MODE == 0) ? ((w & 0xffffu) + (w >> 16)) : w;
-            }
-        }
-        uint32_t excl, total;
-        block_scan_excl_1024(cnt, s_warp, excl, total);
-        const uint32_t npix = (uint32_t)g.H * (uint32_t)g.W;
-        const bool overflow = (MODE == 0) && (total != npix);
-        uint32_t* s_val = s_misc + 8;                       // value (MODE 0) or bin (MODE 1)
-        uint32_t* s_off = s_val + STATS_MAX_RANKS;          // MODE 1: rank offset inside the bin
-        uint32_t* s_cnt = s_off + STATS_MAX_RANKS;          // MODE 1: count of even values in the bin
-        if (!overflow) {
-            for (int qi = 0; qi < g.nranks; qi++) {
-                const uint32_t k = g.ranks[qi];
-                if (k >= excl && k < excl + cnt) {
-                    uint32_t acc = excl;
-                    const uint32_t* hw = hist + tid * 32;
-                    for (int i = 0; i < 32; i++) {
-                        const uint32_t w = hw[i];
-                        if (MODE == 0) {
-                            const uint32_t c0 = w & 0xffffu, c1 = w >> 16;
-                            if (k < acc + c0) { s_val[qi] = (tid * 32 + i) * 2; break; }
-                            acc += c0;
-                            if (k < acc + c1) { s_val[qi] = (tid * 32 + i) * 2 + 1; break; }
-                            acc += c1;
-                        } else {
-                            if (k < acc + w) { s_val[qi] = tid * 32 + i; s_off[qi] = k - acc; s_cnt[qi] = 0; break; }
-                            acc += w;
-                        }
-                    }
-                }
-            }
-        }
-        __syncthreads();
-        if (MODE == 1 && g.nranks > 0) {
-            // second pass: how many pixels equal 2*bin (the even value of each target bin)?
-            uint32_t local[STATS_MAX_RANKS];
-#pragma unroll
-            for (int qi = 0; qi < STATS_MAX_RANKS; qi++) local[qi] = 0;
-            for (int i = tid; i < g.H * g.W; i += STATS_THREADS) {
-                const int rr = i / g.W, cc = i - rr * g.W;
-                const uint32_t v = __ldg(f + (size_t)rr * pitch + cc);
-#pragma unroll
-                for (int qi = 0; qi < STATS_MAX_RANKS; qi++)
-                    if (qi < g.nranks && v == 2u * s_val[qi]) local[qi]++;
-            }
-#pragma unroll
-            for (int qi = 0; qi < STATS_MAX_RANKS; qi++) {
-                if (qi < g.nranks) {
-                    uint32_t s = warp_sum(local[qi]);
-                    if (lane == 0 && s) atomicAdd(&s_cnt[qi], s);
-                }
-            }
-            __syncthreads();
-        }
-        if (tid == 0) {
-            FrameStats& o = stats[slot];
-            o.mn = s_misc[0];
-            o.mx = s_misc[1];
-            o.npix = npix;
-            o.sum = *reinterpret_cast<unsigned long long*>(&s_misc[2]);
-            o.corner_sum = *reinterpret_cast<unsigned long long*>(&s_misc[4]);
-            o.overflow = overflow ? 1u : 0u;
-            if (!overflow)
-                for (int qi = 0; qi < g.nranks; qi++)
-                    o.ostat[qi] = (MODE == 0) ? s_val[qi] : (2u * s_val[qi] + (s_off[qi] >= s_cnt[qi] ? 1u : 0u));
-        }
-        __syncthreads();
-    }
+void launch_refs_from_batch(epid_ctx* ctx, cudaStream_t stream, const uint16_t* base, int n, int H0, int W0, int r0, int c0, FrameRef* refs) {
+    k_refs_from_batch<<<(n + 127) / 128, 128, 0, stream>>>(base, n, H0, W0, r0, c0, refs);
+    ctx->launches++;
 }
 
-// ------------------------------------------------------------------------------------------------ multi-CTA variant
-// The single-CTA kernel above keeps a frame's histogram in shared memory, which ties a frame to one SM.  This
-// variant spreads a frame over HV_PARTS CTAs: each streams a block of rows with 16-byte loads, merges equal values of a warp
-// (__match_any_sync) into a direct-mapped shared-memory cache of histogram bins (first claimant owns a slot, losers go to the global
-// histogram; one global atomic per occupied slot at the end), keeps column sums in registers and writes row sums directly; a
-// second kernel (one CTA per frame) turns the 65536-bin histogram into min / max / sum / order statistics and adds the column
-// partials.  Exact like the single-CTA kernel (32-bit counters, no overflow path).  Views up to 2040 columns.
+// ------------------------------------------------------------------------------------------------ exact histogram path
+// k_hist_view spreads a frame over HV_PARTS CTAs of row blocks, and a view wider than HV_STRIP columns over column strips as well: each
+// CTA streams its rows of its strip with 16-byte loads, counts every pixel through the bin cache of stats.cuh into the frame's global
+// histogram, keeps column sums in registers and writes row sums (accumulates them, when there are several strips).  k_stats_from_hist,
+// one CTA per frame, turns the 65536-bin histogram into min / max / sum / order statistics and adds the column partials.  32-bit
+// counters throughout.
 constexpr int HV_PARTS = 16;
 constexpr int HV_THREADS = 256;
 constexpr int HV_WARPS = HV_THREADS / 32;
-constexpr int HV_SLOTS = 4096;
+// columns of a strip: with the worst misalignment of 7 pixels they fill the 256 vectors of k_hist_view<8>; a multiple of 8, so every
+// strip keeps the view's 16-byte phase
+constexpr int HV_STRIP = 2040;
 
 template <int VPL>
 __global__ void __launch_bounds__(HV_THREADS)
 k_hist_view(const StatsGeom g, const FrameRef* __restrict__ frames, uint32_t* __restrict__ hist, uint32_t* __restrict__ rowsum_out,
             uint32_t* __restrict__ colpart, int wa) {
-    __shared__ uint32_t s_tag[HV_SLOTS];     // value + 1, 0 = free
-    __shared__ uint32_t s_cnt[HV_SLOTS];
+    __shared__ HistCache s_cache;
     extern __shared__ uint32_t s_col[];      // wa column accumulators of the CTA
-    const int fi = blockIdx.y, part = blockIdx.x;
+    const int fi = blockIdx.y, strip = blockIdx.x / HV_PARTS, part = blockIdx.x - strip * HV_PARTS;
+    const int nstrips = gridDim.x / HV_PARTS;
     const FrameRef fr = frames[fi];
-    const uint16_t* __restrict__ f = fr.origin;
+    const uint16_t* __restrict__ f = fr.origin + strip * HV_STRIP;
+    const int W = min(g.W - strip * HV_STRIP, HV_STRIP);
     const int pitch = fr.pitch;
     uint32_t* h = hist + (size_t)fi * 65536;
     const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const bool aligned = (pitch % 8) == 0;
     const int mis = aligned ? (int)((reinterpret_cast<uintptr_t>(f) >> 1) & 7) : 0;
-    for (int i = tid; i < HV_SLOTS; i += HV_THREADS) { s_tag[i] = 0; s_cnt[i] = 0; }
+    hist_cache_init(s_cache);
     for (int i = tid; i < wa; i += HV_THREADS) s_col[i] = 0;
     __syncthreads();
-    auto add = [&](uint32_t v, bool in) {
-        const unsigned m = __match_any_sync(0xffffffffu, in ? v : 0x10000u);
-        if (in && lane == __ffs(m) - 1) {
-            const uint32_t cn = (uint32_t)__popc(m), slot = v & (HV_SLOTS - 1);
-            const uint32_t old = atomicCAS(&s_tag[slot], 0u, v + 1u);
-            if (old == 0u || old == v + 1u) atomicAdd(&s_cnt[slot], cn);
-            else atomicAdd(&h[v], cn);
-        }
-    };
     const int rp = (g.H + HV_PARTS - 1) / HV_PARTS;
     const int r0 = part * rp, r1 = min(g.H, r0 + rp);
     uint32_t csum[VPL][8];
@@ -353,7 +88,7 @@ k_hist_view(const StatsGeom g, const FrameRef* __restrict__ frames, uint32_t* __
             const int col_first = (lane + 32 * k) * 8 - mis;
             uint32_t vm = 0;
 #pragma unroll
-            for (int e = 0; e < 8; e++) { const int cidx = col_first + e; if (cidx >= 0 && cidx < g.W) vm |= 1u << e; }
+            for (int e = 0; e < 8; e++) { const int cidx = col_first + e; if (cidx >= 0 && cidx < W) vm |= 1u << e; }
             valid[k] = vm;
             q[k] = make_uint4(0, 0, 0, 0);
             if (vm) {
@@ -375,14 +110,17 @@ k_hist_view(const StatsGeom g, const FrameRef* __restrict__ frames, uint32_t* __
             for (int e = 0; e < 8; e++) {
                 const uint32_t v = (w4[e >> 1] >> ((e & 1) * 16)) & 0xffffu;
                 const bool in = valid[k] >> e & 1;
-                add(v, in);
+                hist_cache_add(s_cache, h, v, in);
                 if (in) { csum[k][e] += v; rs += v; }
             }
         }
         rs = warp_sum(rs);
-        if (lane == 0 && rowsum_out) rowsum_out[(size_t)fi * g.H + r] = rs;
+        if (lane == 0 && rowsum_out) {
+            if (nstrips > 1) atomicAdd(&rowsum_out[(size_t)fi * g.H + r], rs);
+            else rowsum_out[(size_t)fi * g.H + r] = rs;
+        }
     }
-    // column partials: registers -> CTA accumulators -> one partial row per (frame, part)
+    // column partials: registers -> CTA accumulators -> one partial row per (frame, part), wa columns per strip
 #pragma unroll
     for (int k = 0; k < VPL; k++)
 #pragma unroll
@@ -391,55 +129,26 @@ k_hist_view(const StatsGeom g, const FrameRef* __restrict__ frames, uint32_t* __
             if (ac < wa && csum[k][e]) atomicAdd(&s_col[ac], csum[k][e]);
         }
     __syncthreads();
-    if (colpart) for (int i = tid; i < wa; i += HV_THREADS) colpart[((size_t)fi * HV_PARTS + part) * wa + i] = s_col[i];
-    for (int i = tid; i < HV_SLOTS; i += HV_THREADS) {
-        const uint32_t tg = s_tag[i];
-        if (tg) atomicAdd(&h[tg - 1u], s_cnt[i]);
-    }
+    if (colpart)
+        for (int i = tid; i < wa; i += HV_THREADS) colpart[((size_t)fi * HV_PARTS + part) * nstrips * wa + strip * wa + i] = s_col[i];
+    hist_cache_flush(s_cache, h);
 }
 
-__global__ void __launch_bounds__(256)
+__global__ void __launch_bounds__(HIST_RANK_THREADS)
 k_stats_from_hist(const StatsGeom g, const FrameRef* __restrict__ frames, const uint32_t* __restrict__ hist, const uint32_t* __restrict__ colpart,
                   int wa, FrameStats* __restrict__ stats, uint32_t* __restrict__ colsum_out) {
-    __shared__ uint32_t s_part[256];
-    __shared__ unsigned long long s_wsum[256];
-    __shared__ uint32_t s_first, s_last;
+    __shared__ HistRanks s;
+    __shared__ unsigned long long s_wsum[HIST_RANK_THREADS];
     __shared__ unsigned long long s_corner;
-    __shared__ uint32_t s_val[STATS_MAX_RANKS];
     const int fi = blockIdx.x, tid = threadIdx.x, lane = tid & 31;
-    const uint32_t* h = hist + (size_t)fi * 65536;
     const FrameRef fr = frames[fi];
-    uint32_t cnt = 0, lo_bin = 0xffffffffu, hi_bin = 0;
-    unsigned long long ws = 0;
-    for (int b = tid * 256; b < (tid + 1) * 256; b++) {
-        const uint32_t hb = h[b];
-        cnt += hb;
-        ws += (unsigned long long)hb * (unsigned)b;
-        if (hb) { if (lo_bin == 0xffffffffu) lo_bin = b; hi_bin = b; }
-    }
-    s_part[tid] = cnt;
-    s_wsum[tid] = ws;
-    if (tid == 0) { s_first = 0xffffffffu; s_last = 0; s_corner = 0; }
-    __syncthreads();
-    if (lo_bin != 0xffffffffu) { atomicMin(&s_first, lo_bin); atomicMax(&s_last, hi_bin); }
-    uint32_t excl = 0;
-    for (int k = 0; k < tid; k++) excl += s_part[k];
-    for (int qi = 0; qi < g.nranks; qi++) {
-        const uint32_t k = g.ranks[qi];
-        if (k >= excl && k < excl + cnt) {
-            uint32_t acc = excl;
-            for (int b = tid * 256; b < (tid + 1) * 256; b++) {
-                const uint32_t hb = h[b];
-                if (k < acc + hb) { s_val[qi] = (uint32_t)b; break; }
-                acc += hb;
-            }
-        }
-    }
+    if (tid == 0) s_corner = 0;
+    hist_rank_search(hist + (size_t)fi * 65536, g.ranks, g.nranks, s, s_wsum);
     // corner boxes (core/image.py:881-894)
     if (g.box > 0) {
         const int per = g.box * g.box;
         unsigned long long cs = 0;
-        for (int i = tid; i < 4 * per; i += 256) {
+        for (int i = tid; i < 4 * per; i += HIST_RANK_THREADS) {
             const int b = i / per, o = i - b * per;
             const int y = o / g.box, x = o - y * g.box;
             const int rr = ((b & 2) ? g.H - g.rp - g.box : g.rp) + y;
@@ -449,28 +158,31 @@ k_stats_from_hist(const StatsGeom g, const FrameRef* __restrict__ frames, const 
         cs = warp_sum(cs);
         if (lane == 0 && cs) atomicAdd(&s_corner, cs);
     }
-    // column sums: the parts' partial rows (vector-grid columns) -> view columns
+    // column sums: the parts' partial rows (vector-grid columns of each strip) -> view columns
     if (colsum_out && colpart) {
         const bool aligned = (fr.pitch % 8) == 0;
         const int mis = aligned ? (int)((reinterpret_cast<uintptr_t>(fr.origin) >> 1) & 7) : 0;
-        for (int x = tid; x < g.W; x += 256) {
+        const int row = (g.W + HV_STRIP - 1) / HV_STRIP * wa;
+        for (int x = tid; x < g.W; x += HIST_RANK_THREADS) {
+            const int strip = x / HV_STRIP;
+            const int ac = strip * wa + (x - strip * HV_STRIP) + mis;
             uint32_t sum = 0;
-            for (int p = 0; p < HV_PARTS; p++) sum += colpart[((size_t)fi * HV_PARTS + p) * wa + x + mis];
+            for (int p = 0; p < HV_PARTS; p++) sum += colpart[((size_t)fi * HV_PARTS + p) * row + ac];
             colsum_out[(size_t)fi * g.W + x] = sum;
         }
     }
     __syncthreads();
     if (tid == 0) {
         unsigned long long tot = 0;
-        for (int k = 0; k < 256; k++) tot += s_wsum[k];
+        for (int k = 0; k < HIST_RANK_THREADS; k++) tot += s_wsum[k];
         FrameStats& o = stats[fi];
-        o.mn = s_first;
-        o.mx = s_last;
+        o.mn = s.first;
+        o.mx = s.last;
         o.npix = (uint32_t)g.H * (uint32_t)g.W;
         o.sum = tot;
         o.corner_sum = s_corner;
-        o.overflow = 0;
-        for (int qi = 0; qi < g.nranks; qi++) o.ostat[qi] = s_val[qi];
+        o.inv_certified = 0;
+        for (int qi = 0; qi < g.nranks; qi++) o.ostat[qi] = s.values[qi];
     }
 }
 
@@ -483,20 +195,34 @@ static int ensure_hist_scratch(epid_ctx* ctx, size_t bytes) {
     return EPID_OK;
 }
 
-template <int VPL>
-static int launch_hist_view(cudaStream_t stream, const StatsGeom& g, const FrameRef* d_frames, int cn, uint32_t* hist, uint32_t* rowsum,
-                            uint32_t* colpart, int wa) {
-    k_hist_view<VPL><<<dim3(HV_PARTS, cn), HV_THREADS, sizeof(uint32_t) * wa, stream>>>(g, d_frames, hist, rowsum, colpart, wa);
-    return EPID_OK;
+// launch shape of k_hist_view for views of W columns
+struct HvShape {
+    int strips;      // column strips of HV_STRIP columns
+    int vpl;         // vectors per lane
+    int wa;          // columns of a strip's vector grid
+};
+
+static HvShape hv_shape(int W) {
+    const int sw = W < HV_STRIP ? W : HV_STRIP;
+    const int vpl = ((sw + 7 + 7) / 8 + 31) / 32;
+    return {(W + HV_STRIP - 1) / HV_STRIP, vpl, vpl * 32 * 8};
 }
 
-static int launch_frame_stats_v2(epid_ctx* ctx, cudaStream_t stream, const StatsGeom& g, const FrameRef* d_frames, int n, FrameStats* d_stats,
-                                 uint32_t* d_rowsum, uint32_t* d_colsum) {
-    const int nvec = (g.W + 7 + 7) / 8;
-    const int vpl = (nvec + 31) / 32;
-    const int wa = vpl * 32 * 8;                 // columns of the vector grid
+// wa = 0: no column sums
+static void launch_hist_view(cudaStream_t stream, const StatsGeom& g, const HvShape& hv, const FrameRef* d_frames, int cn, uint32_t* hist,
+                             uint32_t* rowsum, uint32_t* colpart, int wa) {
+    const dim3 grid(HV_PARTS * hv.strips, cn);
+    const size_t smem = sizeof(uint32_t) * wa;
+    if (hv.vpl <= 4) k_hist_view<4><<<grid, HV_THREADS, smem, stream>>>(g, d_frames, hist, rowsum, colpart, wa);
+    else k_hist_view<8><<<grid, HV_THREADS, smem, stream>>>(g, d_frames, hist, rowsum, colpart, wa);
+}
+
+int launch_frame_stats(epid_ctx* ctx, cudaStream_t stream, const StatsGeom& g, const FrameRef* d_frames, int n, FrameStats* d_stats,
+                       uint32_t* d_rowsum, uint32_t* d_colsum) {
+    const HvShape hv = hv_shape(g.W);
     const int chunk = n < 256 ? n : 256;
-    const size_t hist_b = sizeof(uint32_t) * (size_t)chunk * 65536, col_b = sizeof(uint32_t) * (size_t)chunk * HV_PARTS * wa;
+    const size_t hist_b = sizeof(uint32_t) * (size_t)chunk * 65536;
+    const size_t col_b = sizeof(uint32_t) * (size_t)chunk * HV_PARTS * hv.strips * hv.wa;
     int rc = ensure_hist_scratch(ctx, hist_b + col_b + 512);
     if (rc != EPID_OK) return rc;
     uint32_t* hist = (uint32_t*)ctx->hist_scratch;
@@ -505,12 +231,21 @@ static int launch_frame_stats_v2(epid_ctx* ctx, cudaStream_t stream, const Stats
         const int cn = n - c0 < chunk ? n - c0 : chunk;
         EPID_CUDA(cudaMemsetAsync(hist, 0, sizeof(uint32_t) * (size_t)cn * 65536, stream));
         uint32_t* rs = d_rowsum ? d_rowsum + (size_t)c0 * g.H : nullptr;
-        if (vpl <= 4) rc = launch_hist_view<4>(stream, g, d_frames + c0, cn, hist, rs, colpart, wa);
-        else rc = launch_hist_view<8>(stream, g, d_frames + c0, cn, hist, rs, colpart, wa);
-        k_stats_from_hist<<<cn, 256, 0, stream>>>(g, d_frames + c0, hist, colpart, wa, d_stats + c0, d_colsum ? d_colsum + (size_t)c0 * g.W : nullptr);
+        if (rs && hv.strips > 1) EPID_CUDA(cudaMemsetAsync(rs, 0, sizeof(uint32_t) * (size_t)cn * g.H, stream));
+        launch_hist_view(stream, g, hv, d_frames + c0, cn, hist, rs, colpart, hv.wa);
+        k_stats_from_hist<<<cn, HIST_RANK_THREADS, 0, stream>>>(g, d_frames + c0, hist, colpart, hv.wa, d_stats + c0,
+                                                                d_colsum ? d_colsum + (size_t)c0 * g.W : nullptr);
         ctx->launches += 2;
         EPID_CUDA(cudaGetLastError());
     }
+    return EPID_OK;
+}
+
+int launch_frame_histogram(epid_ctx* ctx, cudaStream_t stream, const StatsGeom& g, const FrameRef* d_frames, int n, uint32_t* d_hist) {
+    EPID_CUDA(cudaMemsetAsync(d_hist, 0, sizeof(uint32_t) * (size_t)n * 65536, stream));
+    launch_hist_view(stream, g, hv_shape(g.W), d_frames, n, d_hist, nullptr, nullptr, 0);
+    ctx->launches++;
+    EPID_CUDA(cudaGetLastError());
     return EPID_OK;
 }
 
@@ -523,8 +258,8 @@ static int launch_frame_stats_v2(epid_ctx* ctx, cudaStream_t stream, const Stats
 //   k_inv_stream  IV_PARTS CTAs per frame, one 16-byte load per lane and vector: exact min / max / sum, row sums, column partials and the
 //                 six exact counts #(v < T) by packed u16x2 arithmetic (no atomics in the pixel loop)
 //   k_inv_finish  CTA per frame: combines the parts; #(v < tL) <= rank_prev and #(v <= tU) > rank_next PROVE tL <= percentile <= tU; if the
-//                 resulting intervals of the two distances do not overlap the decision is certified (FrameStats.overflow = 2 + inverted),
-//                 otherwise the frame is listed for the exact histogram path (ostat exact, overflow = 0).
+//                 resulting intervals of the two distances do not overlap the decision is certified (FrameStats.inv_certified = 2 +
+//                 inverted), otherwise the frame is listed for the exact histogram path (ostat exact, inv_certified = 0).
 constexpr int IV_PARTS = 16;
 constexpr int IV_THREADS = 256;
 constexpr int IV_WARPS = IV_THREADS / 32;
@@ -774,7 +509,7 @@ k_inv_finish(const StatsGeom g, const FrameRef* __restrict__ frames, const uint3
     o.npix = npix;
     o.sum = total;
     o.corner_sum = 0;
-    o.overflow = (uint32_t)code;
+    o.inv_certified = (uint32_t)code;
     for (int k = 0; k < STATS_MAX_RANKS; k++) o.ostat[k] = 0;
     if (code == 0) fail_list[atomicAdd(fail_count, 1)] = fi;
 }
@@ -789,7 +524,7 @@ __global__ void k_inv_scatter_ostat(const FrameStats* __restrict__ src, const in
     if (i >= m) return;
     FrameStats& d = dst[list[i]];
     for (int k = 0; k < STATS_MAX_RANKS; k++) d.ostat[k] = src[i].ostat[k];
-    d.overflow = 0;
+    d.inv_certified = 0;
 }
 
 template <int VPL>
@@ -799,13 +534,13 @@ static void launch_inv_stream(cudaStream_t st, bool cols, const StatsGeom& g, co
     else k_inv_stream<VPL, false><<<dim3(IV_PARTS, n), IV_THREADS, 0, st>>>(g, refs, thr, parts, rowsum, nullptr, wa);
 }
 
-// g.ranks = (prev, next) of the low, middle and high percentile; box must be 0.  Returns with d_stats complete: overflow >= 2 carries the
-// certified decision (2 + inverted, ostat unused), overflow == 0 exact ostat from the histogram path.  One host round trip (count of the
-// uncertified frames).
+// g.ranks = (prev, next) of the low, middle and high percentile; box must be 0.  Returns with d_stats complete: inv_certified >= 2 carries
+// the certified decision (2 + inverted, ostat unused), inv_certified == 0 exact ostat from the histogram path.  One host round trip
+// (count of the uncertified frames).
 int launch_frame_stats_inversion(epid_ctx* ctx, cudaStream_t stream, const StatsGeom& g, const FrameRef* d_frames, int n, FrameStats* d_stats,
                                  uint32_t* d_rowsum, uint32_t* d_colsum) {
     if (ctx->stats_exact || g.nranks != 6 || g.box > 0 || g.W > 2040 || g.H < IV_SAMPLE_ROWS || g.W < 8)
-        return launch_frame_stats(ctx, stream, g, d_frames, nullptr, n, d_stats, d_rowsum, d_colsum);
+        return launch_frame_stats(ctx, stream, g, d_frames, n, d_stats, d_rowsum, d_colsum);
     const int nvec = (g.W + 7 + 7) / 8;
     const int vpl = (nvec + 31) / 32;
     const int wa = vpl * 32 * 8;
@@ -842,33 +577,12 @@ int launch_frame_stats_inversion(epid_ctx* ctx, cudaStream_t stream, const Stats
     ctx->stats_uncertified += m;
     if (m > 0) {       // exact order statistics for the frames whose decision could not be certified
         k_inv_gather_refs<<<(m + 127) / 128, 128, 0, stream>>>(d_frames, list + 1, m, refs2);
-        int rc = launch_frame_stats(ctx, stream, g, refs2, nullptr, m, tmp, nullptr, nullptr);
+        int rc = launch_frame_stats(ctx, stream, g, refs2, m, tmp, nullptr, nullptr);
         if (rc != EPID_OK) return rc;
         k_inv_scatter_ostat<<<(m + 127) / 128, 128, 0, stream>>>(tmp, list + 1, m, d_stats);
         ctx->launches += 2;
         EPID_CUDA(cudaGetLastError());
     }
-    return EPID_OK;
-}
-
-static size_t stats_smem_bytes(const StatsGeom& g) {
-    return sizeof(uint32_t) * (size_t)(HIST_WORDS + STATS_THREADS * 8 + g.H + 40 + 8 + 3 * STATS_MAX_RANKS);
-}
-
-int launch_frame_stats(epid_ctx* ctx, cudaStream_t stream, const StatsGeom& g, const FrameRef* d_frames,
-                       const int* d_out_index, int n, FrameStats* d_stats, uint32_t* d_rowsum, uint32_t* d_colsum) {
-    // multi-CTA histogram path for every view it covers (d_out_index is not used by any caller of that path)
-    if (!d_out_index && g.W <= 2040 && g.nranks <= STATS_MAX_RANKS)
-        return launch_frame_stats_v2(ctx, stream, g, d_frames, n, d_stats, d_rowsum, d_colsum);
-    const size_t smem = stats_smem_bytes(g);
-    EPID_SMEM_OPT_IN(ctx, k_frame_stats<0>, 220 * 1024);
-    EPID_SMEM_OPT_IN(ctx, k_frame_stats<1>, 220 * 1024);
-    const int grid = n < ctx->sm_count ? n : ctx->sm_count;
-    k_frame_stats<0><<<grid, STATS_THREADS, smem, stream>>>(g, d_frames, d_out_index, n, d_stats, d_rowsum, d_colsum);
-    // exact fallback for frames whose packed counters overflowed (CTAs of other frames exit at once)
-    k_frame_stats<1><<<grid, STATS_THREADS, smem, stream>>>(g, d_frames, d_out_index, n, d_stats, d_rowsum, d_colsum);
-    ctx->launches += 2;
-    EPID_CUDA(cudaGetLastError());
     return EPID_OK;
 }
 

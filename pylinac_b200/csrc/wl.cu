@@ -21,7 +21,7 @@
 // integer thresholds on g; the BB sample repeats the reference's fp64 operation order (invert, stretch) pixel by pixel.
 //
 // Stages:
-//   k_wl_hist    exact 65536-bin histogram of every frame (warp-aggregated global atomics)
+//   k_wl_hist    exact 65536-bin histogram of every frame (shared-memory bin cache of stats.cuh)
 //   k_wl_front   CTA per frame: inversion decision, _clean_edges loop (percentiles from the histogram, ring min / max, ring
 //                removal), ground / normalize constants, field threshold
 //   k_wl_field   CTA per frame: bounding box of the thresholded field, fill holes inside it, centre of mass
@@ -66,32 +66,19 @@ struct WlFrame {
 __device__ __forceinline__ uint32_t wl_T(const WlFrame& f, uint32_t v) { return f.flip ? f.S - v : v; }
 
 // ------------------------------------------------------------------------------------------------ histogram
-constexpr int WL_HSLOTS = 4096;        // direct-mapped shared-memory cache of histogram bins (slot = value mod 4096)
 constexpr int WL_HPARTS = 8;           // CTAs per frame
+static_assert(WL_THREADS == HIST_RANK_THREADS, "k_wl_front runs hist_rank_search with all its threads");
 
-// Exact histogram.  A CTA streams 1/8 of a frame with 16-byte loads; lanes that hold the same value are merged
-// (__match_any_sync), and the merged count goes to a shared-memory cache in which the first value that claims a slot owns it for
-// the CTA's lifetime -- EPID frames use a narrow band of values locally, so nearly every add stays in shared memory; values that
-// lose a slot go straight to the global histogram.  The cache is flushed with one global atomic per occupied slot.
+// Exact histogram.  A CTA streams 1/8 of a frame with 16-byte loads and counts it through the bin cache of stats.cuh.
 __global__ void __launch_bounds__(256)
 k_wl_hist(const uint16_t* __restrict__ base, int H, int W, uint32_t* __restrict__ hist) {
-    __shared__ uint32_t s_tag[WL_HSLOTS];     // value + 1, 0 = free
-    __shared__ uint32_t s_cnt[WL_HSLOTS];
+    __shared__ HistCache s_cache;
     const int fi = blockIdx.y;
     const uint16_t* f = base + (size_t)fi * H * W;
     uint32_t* h = hist + (size_t)fi * 65536;
     const int lane = threadIdx.x & 31;
-    for (int i = threadIdx.x; i < WL_HSLOTS; i += 256) { s_tag[i] = 0; s_cnt[i] = 0; }
+    hist_cache_init(s_cache);
     __syncthreads();
-    auto add = [&](uint32_t v, bool in) {
-        const unsigned m = __match_any_sync(0xffffffffu, in ? v : 0x10000u);
-        if (in && lane == __ffs(m) - 1) {
-            const uint32_t c = (uint32_t)__popc(m), slot = v & (WL_HSLOTS - 1);
-            const uint32_t old = atomicCAS(&s_tag[slot], 0u, v + 1u);
-            if (old == 0u || old == v + 1u) atomicAdd(&s_cnt[slot], c);
-            else atomicAdd(&h[v], c);
-        }
-    };
     const size_t npx = (size_t)H * W;
     const size_t per = ((npx + WL_HPARTS - 1) / WL_HPARTS + 7) & ~(size_t)7;
     const size_t p0 = (size_t)blockIdx.x * per, p1 = p0 + per < npx ? p0 + per : npx;
@@ -99,7 +86,7 @@ k_wl_hist(const uint16_t* __restrict__ base, int H, int W, uint32_t* __restrict_
     const size_t mis = ((reinterpret_cast<uintptr_t>(f + p0) >> 1) & 7);
     const size_t v0 = p0 + ((8 - mis) & 7) < p1 ? p0 + ((8 - mis) & 7) : p1;
     const size_t nvec = (p1 - v0) >> 3;
-    if (threadIdx.x < 32) add(p0 + lane < v0 ? f[p0 + lane] : 0u, p0 + lane < v0);
+    if (threadIdx.x < 32) hist_cache_add(s_cache, h, p0 + lane < v0 ? f[p0 + lane] : 0u, p0 + lane < v0);
     const size_t nvec32 = (nvec + 31) & ~(size_t)31;            // every lane of a warp takes the same number of trips
     for (size_t k = threadIdx.x; k < ((nvec32 + 255) & ~(size_t)255); k += 256) {
         const bool in = k < nvec;
@@ -108,59 +95,23 @@ k_wl_hist(const uint16_t* __restrict__ base, int H, int W, uint32_t* __restrict_
         const uint32_t w[4] = {q.x, q.y, q.z, q.w};
 #pragma unroll
         for (int t = 0; t < 4; t++) {
-            add(w[t] & 0xffffu, in);
-            add(w[t] >> 16, in);
+            hist_cache_add(s_cache, h, w[t] & 0xffffu, in);
+            hist_cache_add(s_cache, h, w[t] >> 16, in);
         }
     }
     const size_t t0 = v0 + nvec * 8;
-    if (threadIdx.x < 32) add(t0 + lane < p1 ? f[t0 + lane] : 0u, t0 + lane < p1);
+    if (threadIdx.x < 32) hist_cache_add(s_cache, h, t0 + lane < p1 ? f[t0 + lane] : 0u, t0 + lane < p1);
     __syncthreads();
-    for (int i = threadIdx.x; i < WL_HSLOTS; i += 256) {
-        const uint32_t tg = s_tag[i];
-        if (tg) atomicAdd(&h[tg - 1u], s_cnt[i]);
-    }
+    hist_cache_flush(s_cache, h);
 }
 
 // ------------------------------------------------------------------------------------------------ front
 struct WlScan {
-    uint32_t part[WL_THREADS];
-    uint32_t ranks[8], values[8];
-    uint32_t first, last, total;
+    HistRanks q;                       // values of up to 8 raw order statistics + first / last non-empty bin (hist_rank_search)
+    uint32_t ranks[8];
     double d[WL_WARPS];
     uint32_t u[2 * WL_WARPS];
 };
-
-// values of up to 8 raw order statistics (0-based ranks, ascending or not) + first / last non-empty bin, from a 65536-bin histogram
-__device__ inline void wl_hist_query(const volatile uint32_t* hist, WlScan* s, int nr) {
-    const int tid = threadIdx.x;
-    const int per = 65536 / WL_THREADS;
-    uint32_t c = 0, lo_bin = 0xffffffffu, hi_bin = 0;
-    for (int b = tid * per; b < (tid + 1) * per; b++) {
-        const uint32_t hb = hist[b];
-        c += hb;
-        if (hb) { if (lo_bin == 0xffffffffu) lo_bin = b; hi_bin = b; }
-    }
-    s->part[tid] = c;
-    if (tid == 0) { s->first = 0xffffffffu; s->last = 0; }
-    __syncthreads();
-    if (lo_bin != 0xffffffffu) { atomicMin(&s->first, lo_bin); atomicMax(&s->last, hi_bin); }
-    // exclusive prefix of this thread's range (256 partials: a serial sum per thread is cheap enough)
-    uint32_t excl = 0;
-    for (int k = 0; k < tid; k++) excl += s->part[k];
-    if (tid == WL_THREADS - 1) s->total = excl + c;
-    for (int r = 0; r < nr; r++) {
-        const uint32_t rk = s->ranks[r];
-        if (rk >= excl && rk < excl + c) {
-            uint32_t acc = excl;
-            for (int b = tid * per; b < (tid + 1) * per; b++) {
-                const uint32_t hb = hist[b];
-                if (rk < acc + hb) { s->values[r] = b; break; }
-                acc += hb;
-            }
-        }
-    }
-    __syncthreads();
-}
 
 __global__ void __launch_bounds__(WL_THREADS)
 k_wl_front(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, uint32_t* __restrict__ hist_all, WlFrame* wf) {
@@ -171,6 +122,7 @@ k_wl_front(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, ui
     const int H = c.H, W = c.W;
     const uint16_t* f = base + (size_t)fi * H * W;
     uint32_t* hist = hist_all + (size_t)fi * 65536;
+    const volatile uint32_t* hist_v = hist;   // the searches read the histogram that _clean_edges updates in this kernel
     WlFrame& F = wf[fi];
     // ---- check_inversion_by_histogram((0.01, 50, 99.99)) (core/image.py:899-926)
     uint32_t n = (uint32_t)H * (uint32_t)W;
@@ -183,18 +135,18 @@ k_wl_front(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, ui
         }
     }
     __syncthreads();
-    wl_hist_query(hist, &s, 6);
+    hist_rank_search(hist_v, s.ranks, 6, s.q);
     int flip = 0;
     uint32_t S = 0;
     {
         const double qs[3] = {0.01, 50.0, 99.99};
         double p[3];
-        for (int k = 0; k < 3; k++) p[k] = np_lerp((double)s.values[2 * k], (double)s.values[2 * k + 1], pct_plan((int)n, qs[k]).gamma);
+        for (int k = 0; k < 3; k++) p[k] = np_lerp((double)s.q.values[2 * k], (double)s.q.values[2 * k + 1], pct_plan((int)n, qs[k]).gamma);
         flip = fabs(p[1] - p[0]) > fabs(p[1] - p[2]) ? 1 : 0;
-        S = s.first + s.last;                      // invert(): -a + max + min of the uncropped frame
+        S = s.q.first + s.q.last;                      // invert(): -a + max + min of the uncropped frame
     }
     __syncthreads();
-    if (s.first == s.last) {
+    if (s.q.first == s.q.last) {
         if (tid == 0) { F.status = EPID_WL_FLAT_IMAGE; F.flip = 0; F.S = 0; F.crop = 0; F.h = H; F.w = W; F.mn = 0; F.D = 0; F.g_field = 0; F.by0 = H; F.by1 = -1; F.bx0 = W; F.bx1 = -1; }
         return;
     }
@@ -214,9 +166,9 @@ k_wl_front(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, ui
             s.ranks[2] = flip ? n - 1 - r9a : r9a; s.ranks[3] = flip ? n - 1 - r9b : r9b;
         }
         __syncthreads();
-        wl_hist_query(hist, &s, 4);
-        const double t5a = flip ? (double)(S - s.values[0]) : (double)s.values[0], t5b = flip ? (double)(S - s.values[1]) : (double)s.values[1];
-        const double t9a = flip ? (double)(S - s.values[2]) : (double)s.values[2], t9b = flip ? (double)(S - s.values[3]) : (double)s.values[3];
+        hist_rank_search(hist_v, s.ranks, 4, s.q);
+        const double t5a = flip ? (double)(S - s.q.values[0]) : (double)s.q.values[0], t5b = flip ? (double)(S - s.q.values[1]) : (double)s.q.values[1];
+        const double t9a = flip ? (double)(S - s.q.values[2]) : (double)s.q.values[2], t9b = flip ? (double)(S - s.q.values[3]) : (double)s.q.values[3];
         const double near_min = np_lerp(t5a, t5b, g5), near_max = np_lerp(t9a, t9b, g9);
         const double img_range = near_max - near_min;
         // min / max of the 2-pixel border of the current view (T domain)
@@ -269,9 +221,9 @@ k_wl_front(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, ui
         s.ranks[2] = flip ? n - 1 - r9a : r9a; s.ranks[3] = flip ? n - 1 - r9b : r9b;
     }
     __syncthreads();
-    wl_hist_query(hist, &s, 4);
+    hist_rank_search(hist_v, s.ranks, 4, s.q);
     if (tid == 0) {
-        const uint32_t tmin = flip ? S - s.last : s.first, tmax = flip ? S - s.first : s.last;
+        const uint32_t tmin = flip ? S - s.q.last : s.q.first, tmax = flip ? S - s.q.first : s.q.last;
         const uint32_t D = tmax - tmin;
         F.status = D == 0 ? EPID_WL_FLAT_IMAGE : EPID_WL_OK;
         F.flip = flip;
@@ -286,7 +238,7 @@ k_wl_front(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, ui
         if (D) {
             double v[4];
             for (int k = 0; k < 4; k++) {
-                const uint32_t t = flip ? S - s.values[k] : s.values[k];
+                const uint32_t t = flip ? S - s.q.values[k] : s.q.values[k];
                 v[k] = (double)(t - tmin) / (double)D;              // normalized pixel values
             }
             const double pmin = np_lerp(v[0], v[1], g5), pmax = np_lerp(v[2], v[3], g9);

@@ -92,8 +92,9 @@ def test_percentile_sweep_equals_numpy(ctx, shape):
 
 
 # ------------------------------------------------------------------------------------------------ b. paths and shapes
-def test_histogram_kernel_widths_and_single_cta_kernel(ctx):
-    """k_hist_view with 4 and 8 vectors per lane (W <= 1010, 1011 .. 2040), the single-CTA kernel (W > 2040) up to 4096 columns."""
+def test_histogram_kernel_widths_and_column_strips(ctx):
+    """k_hist_view with 4 and 8 vectors per lane (W <= 1010, 1011 .. 2040), and views wider than 2040 columns cut into strips of 2040
+    columns, up to 4096."""
     rng = np.random.default_rng(1)
     for h, w in [(37, 1000), (33, 1010), (41, 1011), (29, 1024), (23, 1500), (17, 2040), (17, 2041), (64, 4096), (4096, 16), (300, 2100)]:
         frames = rng.integers(0, 65536, (2, h, w), dtype=np.uint16)
@@ -113,6 +114,22 @@ def test_column_offsets_and_unaligned_pitch(ctx):
         frames = rng.integers(0, 65536, (2, 21, w), dtype=np.uint16)
         _check(ctx, frames, f"pitch {w}")
         _check(ctx, frames, f"pitch {w}, offset 3", view=(1, 3, 19, w - 5))
+
+
+def test_histogram_of_a_view_wider_than_4096_columns(ctx):
+    """frame_histogram takes views wider than frame_stats' 4096 columns (three 2040-column strips, the last one partial)."""
+    from pylinac_b200 import _native as nat
+
+    rng = np.random.default_rng(10)
+    frames = rng.integers(0, 65536, (2, 8, 5008), dtype=np.uint16)
+    frames[1] = rng.integers(30000, 30100, (8, 5008))
+    b = nat.Batch.upload(ctx, frames)
+    try:
+        hist = nat.frame_histogram(ctx, b, view=(0, 3, 8, 5000))
+    finally:
+        b.free()
+    for i in range(2):
+        np.testing.assert_array_equal(hist[i], np.bincount(frames[i, :, 3:5003].ravel(), minlength=65536), err_msg=str(i))
 
 
 def test_degenerate_views(ctx):
@@ -141,9 +158,9 @@ def test_constant_two_value_and_extreme_frames(ctx):
 @pytest.mark.parametrize("value", [1000, 1001, "both"])
 @pytest.mark.parametrize("w", [4096, 2040])
 def test_more_than_65535_equal_pixels(ctx, value, w):
-    """More than 65535 pixels of one even or odd value: the single-CTA kernel's packed 16-bit counter overflows and the frame
-    is re-run with 32-bit counters (k_frame_stats<1>); the multi-CTA kernel (W <= 2040) counts in 32 bits throughout.  Ranks
-    at both ends of the repeated value and of its odd / even neighbour are read."""
+    """More than 65535 pixels of one even or odd value would overflow a 16-bit bin counter; k_hist_view counts in 32 bits, in
+    one column strip (W = 2040) and in three (W = 4096).  Ranks at both ends of the repeated value and of its odd / even
+    neighbour are read."""
     h = 64
     n = h * w
     rng = np.random.default_rng(w + (value if isinstance(value, int) else 7))
