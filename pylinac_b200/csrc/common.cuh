@@ -79,6 +79,8 @@ struct epid_ctx {
     int* h_flags = nullptr;              // 64 page-locked, device-mapped ints: [0] deferred count written by k_pf_collect_deferred
     // dynamic shared memory opt-ins already made ON THIS DEVICE (cudaFuncSetAttribute is per device; one ctx per device)
     std::unordered_map<const void*, size_t> smem_optin;
+    // CTAs per SM of kernels launched one resident wave deep (resident_grid)
+    std::unordered_map<const void*, int> ctas_per_sm;
 };
 
 constexpr size_t EPID_BATCH_PAD = 256;
@@ -107,6 +109,20 @@ inline int smem_opt_in(epid_ctx* ctx, K* kernel, size_t bytes) {
     return EPID_OK;
 }
 #define EPID_SMEM_OPT_IN(ctx, kernel, bytes) do { int _rc = ::epid::smem_opt_in(ctx, kernel, bytes); if (_rc != EPID_OK) return _rc; } while (0)
+
+// *grid = min(items, CTAs of `kernel` resident on the device at once) for a kernel that loops over its items; a kernel is always
+// launched with the same block size and dynamic shared memory (the per-SM figure is remembered per ctx, i.e. per device)
+template <class K>
+inline int resident_grid(epid_ctx* ctx, K* kernel, int threads, size_t smem, long long items, int* grid) {
+    int& per_sm = ctx->ctas_per_sm[(const void*)kernel];
+    if (per_sm == 0) {
+        EPID_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+        if (per_sm < 1) per_sm = 1;
+    }
+    const long long cap = (long long)per_sm * ctx->sm_count;
+    *grid = (int)(items < cap ? (items > 0 ? items : 1) : cap);
+    return EPID_OK;
+}
 
 // ------------------------------------------------------------------------------------------------ device helpers
 #ifdef __CUDACC__

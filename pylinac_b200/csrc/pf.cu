@@ -176,18 +176,13 @@ k_pf_profile(const PfConst* __restrict__ cc, PfFrame* fr, const uint32_t* __rest
 
 // ------------------------------------------------------------------------------------------------ windows
 // One warp per (leaf, picket) window.  Canonical window coordinates: i in [0, nr) across the leaf (the axis the
-// median collapses), j in [0, nc) along leaf travel.
-__global__ void __launch_bounds__(WIN_WARPS * 32)
-k_pf_windows(const PfConst* __restrict__ cc, const FrameRef* __restrict__ frames, PfFrame* fr, PfWin* __restrict__ wins, int todo_only) {
-    __shared__ __align__(16) uint16_t s_px[WIN_WARPS][WIN_CAP_PX];     // staged g values; later aliased by the fp64 profile
-    __shared__ uint32_t s_m2[WIN_WARPS][WIN_MAX_NC];
-    const int fi = blockIdx.y;
-    const PfConst& c = *cc;
-    PfFrame& f = fr[fi];
+// median collapses), j in [0, nc) along leaf travel.  This part: the windows k_pf_windows_fast left (valid == -1) in the in-view leaf
+// slots part, part + nparts, ... of frame fi.
+__device__ __forceinline__ void windows_generic_part(const PfConst& c, const FrameRef* __restrict__ frames, PfFrame& f, PfWin* __restrict__ wins,
+                                                     int fi, int part, int nparts, uint16_t (*s_px)[WIN_CAP_PX], uint32_t (*s_m2)[WIN_MAX_NC]) {
     if (f.status != EPID_PF_OK) return;
-    if (todo_only && !f.todo) return;
     const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int li = blockIdx.x; li < f.n_inview; li += gridDim.x) {   // in-view leaf slot
+    for (int li = part; li < f.n_inview; li += nparts) {   // in-view leaf slot
     const int H = c.H, W = c.W;
     const int orient = f.orientation;
     const int leaf = f.inview[li];
@@ -204,7 +199,7 @@ k_pf_windows(const PfConst* __restrict__ cc, const FrameRef* __restrict__ frames
 
     for (int pk = wid; pk < f.n_pickets; pk += WIN_WARPS) {
         PfWin& out = wins[((size_t)fi * PF_L + li) * PF_P + pk];
-        if (todo_only && out.valid != -1) continue;   // already done by k_pf_windows_fast
+        if (out.valid != -1) continue;   // already done by k_pf_windows_fast
         const double pidx = (double)f.picket_idx[pk];
         const double spacing = f.spacing;
         // _get_mlc_window (picketfence.py:859-886): python int() truncates toward zero
@@ -398,6 +393,15 @@ k_pf_windows(const PfConst* __restrict__ cc, const FrameRef* __restrict__ frames
         __syncwarp();
     }
     }   // leaf slots
+}
+
+// one resident wave; item = frame x nparts + part, for the frames k_pf_windows_fast left work in (PfFrame.todo)
+__global__ void __launch_bounds__(WIN_WARPS * 32)
+k_pf_windows(const PfConst* __restrict__ cc, const FrameRef* __restrict__ frames, PfFrame* fr, PfWin* __restrict__ wins, int n, int nparts) {
+    __shared__ __align__(16) uint16_t s_px[WIN_WARPS][WIN_CAP_PX];     // staged g values; later aliased by the fp64 profile
+    __shared__ uint32_t s_m2[WIN_WARPS][WIN_MAX_NC];
+    pf_walk_items(blockIdx.x, gridDim.x, n * nparts, [&](int it) { return fr[it / nparts].todo != 0; },
+                  [&](int it) { windows_generic_part(*cc, frames, fr[it / nparts], wins, it / nparts, it % nparts, nparts, s_px, s_m2); });
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -726,8 +730,11 @@ static int pf_run(epid_ctx* ctx, cudaStream_t stream, const uint16_t* d_frames, 
         rc = launch_pf_windows_fast(ctx, stream, w.cst, w.refs, w.fr, w.wins, n);
         if (rc != EPID_OK) return rc;
         if (tm) { rc = tm->mark(stream, PF_STAGE_WINDOWS); if (rc != EPID_OK) return rc; }
-        dim3 grid(p->n_leaves < 8 ? p->n_leaves : 8, n);   // exits at once unless the fast kernel left work (PfFrame.todo)
-        k_pf_windows<<<grid, WIN_WARPS * 32, 0, stream>>>(w.cst, w.refs, w.fr, w.wins, 1);
+        const int nparts = p->n_leaves < 8 ? p->n_leaves : 8;
+        int grid = 0;
+        rc = resident_grid(ctx, k_pf_windows, WIN_WARPS * 32, 0, (long long)n * nparts, &grid);
+        if (rc != EPID_OK) return rc;
+        k_pf_windows<<<grid, WIN_WARPS * 32, 0, stream>>>(w.cst, w.refs, w.fr, w.wins, n, nparts);
         ctx->launches++;
         if (tm) { rc = tm->mark(stream, PF_STAGE_WINDOWS_GENERIC); if (rc != EPID_OK) return rc; }
     }

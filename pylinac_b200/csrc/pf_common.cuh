@@ -68,6 +68,19 @@ struct alignas(16) PfWinRec {              // one per window, 400 bytes
 };
 static_assert(sizeof(PfWinRec) == 400, "PfWinRec layout");
 
+// Work loop of a window kernel launched one resident wave deep: the calling warp takes the items first, first + stride, ... < nitems
+// and calls body(item) for those where gate(item) holds.  The gates of 32 items are read at once (one per lane) into a ballot
+// mask, so the items without work -- most of them when another kernel took their frames -- cost no dependent load each.  With
+// first = blockIdx.x and stride = gridDim.x every warp of the CTA walks the same items (gates must not change during the kernel).
+template <class Gate, class Body>
+__device__ __forceinline__ void pf_walk_items(int first, int stride, int nitems, Gate gate, Body body) {
+    const int lane = threadIdx.x & 31;
+    for (int base = first; base < nitems; base += 32 * stride) {
+        const int it = base + lane * stride;
+        for (uint32_t m = __ballot_sync(0xffffffffu, it < nitems && gate(it)); m; m &= m - 1) body(base + (__ffs(m) - 1) * stride);
+    }
+}
+
 // noise flag (_has_noise), corner inversion, D, median in g units for one frame from its statistics.
 // check_noise: evaluate the noise criterion (and count noisy frames in counters[0]); post_filter: statistics were taken
 // on an already inverted + filtered copy, only D / median are refreshed.

@@ -15,11 +15,13 @@ __device__ __forceinline__ unsigned long long mad_wide_u32(uint32_t a, uint32_t 
 }
 
 // Batcher merge-exchange network (valid for any N) as a compile-time comparator list.  The list is applied through template
-// arguments, so every array index is a constant and the sorted values stay in registers (written as nested loops the compiler left
-// the array in local memory: LDL / STL around every comparator).
+// arguments, so every array index is a constant and the values stay in registers (written as nested loops the compiler left the
+// array in local memory: LDL / STL around every comparator).
+enum : signed char { NET_BOTH = 0, NET_MIN = 1, NET_MAX = 2 };      // comparator kind: which of its outputs is written
 struct NetList {
     int n;
-    short a[640], b[640];
+    short a[640], b[640];      // a < b: a receives the minimum, b the maximum
+    signed char k[640];
 };
 constexpr NetList batcher_net(int N) {
     NetList L{};
@@ -30,59 +32,74 @@ constexpr NetList batcher_net(int N) {
                     if (i <= N - j - k - 1 && (i + j) / (2 * p) == (i + j + k) / (2 * p)) {
                         L.a[L.n] = (short)(i + j);
                         L.b[L.n] = (short)(i + j + k);
+                        L.k[L.n] = NET_BOTH;
                         L.n++;
                     }
     return L;
+}
+// L restricted to what reaches the wires in `live` (bit w: wire w is read after the network, N <= 64).  Walked backwards, a
+// comparator with no live output is dropped, one with a single live output computes only that one (one VIMNMX instead of two),
+// and the inputs of every kept comparator become live.
+constexpr NetList prune_net(const NetList& L, unsigned long long live) {
+    signed char kind[640] = {};
+    for (int i = L.n - 1; i >= 0; i--) {
+        const unsigned long long ma = 1ull << L.a[i], mb = 1ull << L.b[i];
+        const bool la = (live & ma) != 0, lb = (live & mb) != 0;
+        kind[i] = la && lb ? NET_BOTH : (la ? NET_MIN : (lb ? NET_MAX : (signed char)-1));
+        if (la || lb) live |= ma | mb;
+    }
+    NetList P{};
+    for (int i = 0; i < L.n; i++)
+        if (kind[i] >= 0) {
+            P.a[P.n] = L.a[i];
+            P.b[P.n] = L.b[i];
+            P.k[P.n] = kind[i];
+            P.n++;
+        }
+    return P;
+}
+// Batcher network on N wires pruned to the two wires O1, O2 (a selection network for those two order statistics)
+template <int N, int O1, int O2>
+struct SelectNet {
+    static constexpr NetList L = prune_net(batcher_net(N), (1ull << O1) | (1ull << O2));
+};
+
+template <int A, int B, int K, int N>
+__device__ __forceinline__ void cmpswap_u16x2(uint32_t (&r)[N]) {
+    const uint32_t a = r[A], b = r[B];
+    if constexpr (K != NET_MAX) r[A] = __vminu2(a, b);
+    if constexpr (K != NET_MIN) r[B] = __vmaxu2(a, b);
+}
+template <class Net, int N, int... I>
+__device__ __forceinline__ void apply_net_u16x2(uint32_t (&r)[N], std::integer_sequence<int, I...>) {
+    (cmpswap_u16x2<Net::L.a[I], Net::L.b[I], Net::L.k[I], N>(r), ...);
 }
 template <int N>
 struct BatcherNet {
     static constexpr NetList L = batcher_net(N);
 };
-
-template <int A, int B, int N>
-__device__ __forceinline__ void cmpswap_u16x2(uint32_t (&r)[N]) {
-    const uint32_t a = r[A], b = r[B];
-    r[A] = __vminu2(a, b);
-    r[B] = __vmaxu2(a, b);
-}
-template <int N, int... I>
-__device__ __forceinline__ void apply_net_u16x2(uint32_t (&r)[N], std::integer_sequence<int, I...>) {
-    (cmpswap_u16x2<BatcherNet<N>::L.a[I], BatcherNet<N>::L.b[I], N>(r), ...);
-}
-// ascending in both 16-bit halves independently
+// ascending in both 16-bit halves independently.  Not pruned for the medians: with every index a constant the compiler already
+// drops the comparators that do not reach the outputs read (60 VIMNMX per column pair at 13 rows either way), and the pruned
+// list, scheduled differently, made the non-inlined callers (pair_median_any) spill more.
 template <int N>
 __device__ __forceinline__ void sort_net_u16x2(uint32_t (&r)[N]) {
-    apply_net_u16x2<N>(r, std::make_integer_sequence<int, BatcherNet<N>::L.n>{});
+    apply_net_u16x2<BatcherNet<N>>(r, std::make_integer_sequence<int, BatcherNet<N>::L.n>{});
 }
 
-template <int A, int B, int N>
+template <int A, int B, int K, int N>
 __device__ __forceinline__ void cmpswap_u64(unsigned long long (&r)[N]) {
     const unsigned long long a = r[A], b = r[B];
-    r[A] = a < b ? a : b;
-    r[B] = a < b ? b : a;
+    if constexpr (K != NET_MAX) r[A] = a < b ? a : b;
+    if constexpr (K != NET_MIN) r[B] = a < b ? b : a;
 }
-template <int N, int... I>
+template <class Net, int N, int... I>
 __device__ __forceinline__ void apply_net_u64(unsigned long long (&r)[N], std::integer_sequence<int, I...>) {
-    (cmpswap_u64<BatcherNet<N>::L.a[I], BatcherNet<N>::L.b[I], N>(r), ...);
+    (cmpswap_u64<Net::L.a[I], Net::L.b[I], Net::L.k[I], N>(r), ...);
 }
-template <int A, int B, int N>
-__device__ __forceinline__ void cmpswap_f64(double (&r)[N]) {
-    const double a = r[A], b = r[B];
-    r[A] = fmin(a, b);
-    r[B] = fmax(a, b);
-}
-template <int N, int... I>
-__device__ __forceinline__ void apply_net_f64(double (&r)[N], std::integer_sequence<int, I...>) {
-    (cmpswap_f64<BatcherNet<N>::L.a[I], BatcherNet<N>::L.b[I], N>(r), ...);
-}
-template <int N>
-__device__ __forceinline__ void sort_net_f64(double (&r)[N]) {
-    apply_net_f64<N>(r, std::make_integer_sequence<int, BatcherNet<N>::L.n>{});
-}
-
-template <int N>
-__device__ __forceinline__ void sort_net_u64(unsigned long long (&r)[N]) {
-    apply_net_u64<N>(r, std::make_integer_sequence<int, BatcherNet<N>::L.n>{});
+template <int N, int O1, int O2>
+__device__ __forceinline__ void select_net_u64(unsigned long long (&r)[N]) {
+    using Net = SelectNet<N, O1, O2>;
+    apply_net_u64<Net>(r, std::make_integer_sequence<int, Net::L.n>{});
 }
 
 // 2 * median over exactly N rows of the travel-sample pair in word `t`: (va + vb) per half
@@ -132,71 +149,6 @@ static __device__ __noinline__ uint2 pair_median_any(const uint16_t* __restrict_
             else pair_median_padded<64>(px, S, nr, t, m_lo, m_hi);
     }
     return make_uint2(m_lo, m_hi);
-}
-
-// ---- variants that also return the packed extreme over the rows (maximum, or minimum when want_min) of the two columns
-template <int N>
-__device__ __forceinline__ void pair_median_ext_exact(const uint16_t* __restrict__ px, int S, int t, bool want_min, uint32_t& m_lo, uint32_t& m_hi,
-                                                      uint32_t& ext2) {
-    uint32_t r[N];
-#pragma unroll
-    for (int i = 0; i < N; i++) r[i] = *reinterpret_cast<const uint32_t*>(px + i * S + 2 * t);
-    uint32_t e = r[0];
-    if (want_min) {
-#pragma unroll
-        for (int i = 1; i < N; i++) e = __vminu2(e, r[i]);
-    } else {
-#pragma unroll
-        for (int i = 1; i < N; i++) e = __vmaxu2(e, r[i]);
-    }
-    ext2 = e;
-    sort_net_u16x2<N>(r);
-    const uint32_t va = r[(N - 1) / 2], vb = r[N / 2];
-    m_lo = (va & 0xffffu) + (vb & 0xffffu);
-    m_hi = (va >> 16) + (vb >> 16);
-}
-
-template <int NRP>
-__device__ __forceinline__ void pair_median_ext_padded(const uint16_t* __restrict__ px, int S, int nr, int t, bool want_min, uint32_t& m_lo,
-                                                       uint32_t& m_hi, uint32_t& ext2) {
-    uint32_t r[NRP];
-    uint32_t e = want_min ? 0xffffffffu : 0u;
-#pragma unroll
-    for (int i = 0; i < NRP; i++) {
-        r[i] = 0xffffffffu;
-        if (i < nr) {
-            r[i] = *reinterpret_cast<const uint32_t*>(px + i * S + 2 * t);
-            e = want_min ? __vminu2(e, r[i]) : __vmaxu2(e, r[i]);
-        }
-    }
-    ext2 = e;
-    sort_net_u16x2<NRP>(r);
-    const int k1 = (nr - 1) / 2, k2 = nr / 2;
-    uint32_t va = 0, vb = 0;
-#pragma unroll
-    for (int i = 0; i < NRP; i++) {
-        if (i == k1) va = r[i];
-        if (i == k2) vb = r[i];
-    }
-    m_lo = (va & 0xffffu) + (vb & 0xffffu);
-    m_hi = (va >> 16) + (vb >> 16);
-}
-
-static __device__ __noinline__ uint3 pair_median_ext_any(const uint16_t* __restrict__ px, int S, int nr, int t, bool want_min) {
-    uint32_t m_lo = 0, m_hi = 0, e = 0;
-    switch (nr) {
-#define EPID_MED_CASE(N) case N: pair_median_ext_exact<N>(px, S, t, want_min, m_lo, m_hi, e); break;
-        EPID_MED_CASE(6) EPID_MED_CASE(7) EPID_MED_CASE(8) EPID_MED_CASE(9) EPID_MED_CASE(10) EPID_MED_CASE(11)
-        EPID_MED_CASE(12) EPID_MED_CASE(13) EPID_MED_CASE(14) EPID_MED_CASE(15) EPID_MED_CASE(16) EPID_MED_CASE(17)
-        EPID_MED_CASE(18) EPID_MED_CASE(19) EPID_MED_CASE(20) EPID_MED_CASE(21) EPID_MED_CASE(22) EPID_MED_CASE(23)
-        EPID_MED_CASE(24) EPID_MED_CASE(25) EPID_MED_CASE(26) EPID_MED_CASE(27) EPID_MED_CASE(28) EPID_MED_CASE(29)
-        EPID_MED_CASE(30) EPID_MED_CASE(31) EPID_MED_CASE(32)
-#undef EPID_MED_CASE
-        default:
-            if (nr < 6) pair_median_ext_padded<8>(px, S, nr, t, want_min, m_lo, m_hi, e);
-            else pair_median_ext_padded<32>(px, S, nr, t, want_min, m_lo, m_hi, e);      // not reached: nr <= 32 on this path
-    }
-    return make_uint3(m_lo, m_hi, e);
 }
 
 // serial FWXM analysis of one window's median profile m[0..nc) (2 * median in g units), lane-private.

@@ -3,7 +3,8 @@
 // Reference semantics: PicketFence._get_mlc_window / _is_mlc_peak_in_window (picketfence.py:847-886) and
 // MLCValue.get_peak_positions (picketfence.py:1605-1628) -> FWXMProfilePhysical.field_edge_idx (core/profile.py:602-611).
 //
-// One warp per window, 16 windows in flight per CTA (2 CTAs per SM), the windows of a frame spread over gridDim.x CTAs.
+// One warp per window, 16 windows in flight per CTA (2 CTAs per SM), the windows of a frame spread over W2_GRID_X parts; the grid
+// is one resident wave of CTAs that loop over the (frame, part) items of the frames the two-kernel path did not take.
 //   1. stage the window as exact integers g (ground / invert folded in) into shared memory, canonical layout
 //      px[i * S + jj]: i across the leaf (the axis np.median collapses), jj along leaf travel.  Up-Down frames are staged
 //      with 128-bit loads on the frame's aligned 8-pixel grid, all loads of a window in flight at once (jj = column - cs,
@@ -86,14 +87,10 @@ __device__ __forceinline__ void row_std_stats(const uint16_t* __restrict__ px, i
     sd_med = (nr & 1) ? med_a : (med_a + med_b) / 2.0;
 }
 
-__global__ void __launch_bounds__(W2_WARPS * 32, 2)
-k_pf_windows_fast(const PfConst* __restrict__ cc, const FrameRef* __restrict__ frames, PfFrame* fr, PfWin* __restrict__ wins) {
-    extern __shared__ __align__(16) unsigned char smraw[];
-    __shared__ int s_geo[4];     // status, slot bytes, bytes of the staging part, active warps
-    const int fi = blockIdx.y;
-    const PfConst& c = *cc;
+// part `part` (of W2_GRID_X) of the windows of frame fi, with the whole CTA
+__device__ __forceinline__ void windows_fast_part(const PfConst& c, const FrameRef* __restrict__ frames, PfFrame* fr, PfWin* __restrict__ wins,
+                                                  int fi, int part, unsigned char* smraw, int* s_geo) {
     PfFrame& f = fr[fi];
-    if (f.win2) return;          // the two-kernel window path owns this frame (pf_windows2.cu)
     const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int H = c.H, W = c.W;
     const double dpmm = c.p.dpmm;
@@ -123,7 +120,7 @@ k_pf_windows_fast(const PfConst* __restrict__ cc, const FrameRef* __restrict__ f
     const int total = f.n_inview * np;
     const int active = s_geo[3];
     if (active == 0) {           // windows too large for the fast path: all of them go to the generic kernel
-        for (int widx = blockIdx.x * blockDim.x + threadIdx.x; widx < total; widx += gridDim.x * blockDim.x) {
+        for (int widx = part * blockDim.x + threadIdx.x; widx < total; widx += W2_GRID_X * blockDim.x) {
             const int li = widx / np, pk = widx - li * np;
             wins[((size_t)fi * PF_L + li) * PF_P + pk].valid = -1;
         }
@@ -146,7 +143,7 @@ k_pf_windows_fast(const PfConst* __restrict__ cc, const FrameRef* __restrict__ f
     const bool aligned = (frf.pitch & 7) == 0;
     const int mis = (int)((reinterpret_cast<uintptr_t>(frf.origin) >> 1) & 7);
 
-    for (int widx = blockIdx.x * active + wid; widx < total; widx += gridDim.x * active) {
+    for (int widx = part * active + wid; widx < total; widx += W2_GRID_X * active) {
         const int li = widx / np, pk = widx - li * np;
         const int leaf = f.inview[li];
         const double lw_px = c.p.leaf_width_mm[leaf] * dpmm;
@@ -279,7 +276,7 @@ k_pf_windows_fast(const PfConst* __restrict__ cc, const FrameRef* __restrict__ f
         }
         {
             // the warp's next window: pull its rows towards L2 / L1 now, so that its staging loads do not wait for HBM
-            const int nwidx = widx + gridDim.x * active;
+            const int nwidx = widx + W2_GRID_X * active;
             if (nwidx < total && orient == 0) {
                 const int nli = nwidx / np, npk = nwidx - nli * np;
                 const int nleaf = f.inview[nli];
@@ -471,11 +468,24 @@ k_pf_windows_fast(const PfConst* __restrict__ cc, const FrameRef* __restrict__ f
     }
 }
 
+// one resident wave; item = frame x W2_GRID_X + part, skipped for the frames the two-kernel window path owns (pf_windows2.cu)
+__global__ void __launch_bounds__(W2_WARPS * 32, 2)
+k_pf_windows_fast(const PfConst* __restrict__ cc, const FrameRef* __restrict__ frames, PfFrame* fr, PfWin* __restrict__ wins, int n) {
+    extern __shared__ __align__(16) unsigned char smraw[];
+    __shared__ int s_geo[4];     // status, slot bytes, bytes of the staging part, active warps
+    pf_walk_items(blockIdx.x, gridDim.x, n * W2_GRID_X, [&](int it) { return fr[it / W2_GRID_X].win2 == 0; }, [&](int it) {
+        windows_fast_part(*cc, frames, fr, wins, it / W2_GRID_X, it % W2_GRID_X, smraw, s_geo);
+        __syncthreads();     // the next item reuses s_geo and the slots
+    });
+}
+
 int launch_pf_windows_fast(epid_ctx* ctx, cudaStream_t stream, const PfConst* cst, const FrameRef* refs, PfFrame* fr, PfWin* wins, int n) {
     const size_t smem = W2_POOL;
     EPID_SMEM_OPT_IN(ctx, k_pf_windows_fast, smem);
-    dim3 grid(W2_GRID_X, n);
-    k_pf_windows_fast<<<grid, W2_WARPS * 32, smem, stream>>>(cst, refs, fr, wins);
+    int grid = 0;
+    int rc = resident_grid(ctx, k_pf_windows_fast, W2_WARPS * 32, smem, (long long)n * W2_GRID_X, &grid);
+    if (rc != EPID_OK) return rc;
+    k_pf_windows_fast<<<grid, W2_WARPS * 32, smem, stream>>>(cst, refs, fr, wins, n);
     ctx->launches++;
     EPID_CUDA(cudaGetLastError());
     return EPID_OK;

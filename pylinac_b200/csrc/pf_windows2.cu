@@ -319,25 +319,23 @@ k_pf_win_medians(const PfConst* __restrict__ cc, const FrameRef* __restrict__ fr
     }
 }
 
-// max, and the two middle order statistics of the nr keys a thread reads through key(i) (i < N slots, slots >= nr padded)
-// (an fp64 network on DMNMX pairs would also be exact: the numerators are exact as doubles)
+// max, and the two middle order statistics of the nr <= N keys a thread reads through key(i) (an fp64 network on DMNMX pairs
+// would also be exact: the numerators are exact as doubles).  The p = N - nr padding slots hold ceil(p / 2) zeros and floor(p / 2)
+// ~0, so the middles of the keys are the middles of all N slots, on the fixed wires N / 2 - 1 and N / 2 (both N / 2 for odd nr):
+// a pruned network.
 template <int N, class F>
 __device__ __forceinline__ void rank_keys(F key, int nr, unsigned long long& kmax, unsigned long long& ka, unsigned long long& kb) {
+    const int zeros_end = nr + (N - nr + 1) / 2;
     unsigned long long r[N];
     kmax = 0;
 #pragma unroll
     for (int i = 0; i < N; i++) {
-        r[i] = i < nr ? key(i) : ~0ull;
-        if (i < nr && r[i] > kmax) kmax = r[i];
+        r[i] = i < nr ? key(i) : (i < zeros_end ? 0ull : ~0ull);
+        if (i < nr) kmax = max(kmax, r[i]);
     }
-    sort_net_u64<N>(r);
-    const int k1 = (nr - 1) / 2, k2 = nr / 2;
-    ka = 0; kb = 0;
-#pragma unroll
-    for (int i = 0; i < N; i++) {
-        if (i == k1) ka = r[i];
-        if (i == k2) kb = r[i];
-    }
+    select_net_u64<N, N / 2 - 1, N / 2>(r);
+    ka = (nr & 1) ? r[N / 2] : r[N / 2 - 1];
+    kb = r[N / 2];
 }
 
 __global__ void __launch_bounds__(WB_THREADS, 4)
