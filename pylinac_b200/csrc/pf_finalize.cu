@@ -7,8 +7,8 @@
 //
 // Everything that scales with the number of measurements runs data-parallel: thread per (leaf, picket) pair for the table
 // and the errors (the table index of a pair is its leaf row's offset plus a popcount over the row's validity mask), warp per
-// picket for the line fits and the width statistics, block reductions for the aggregates.  Only O(leaves) and O(pickets)
-// bookkeeping is left to one thread.
+// picket for the line fits and the width statistics, block reductions for the aggregates.  The O(leaves) and O(pickets)
+// bookkeeping (kiss-count median, row offsets, fit check, dist2cax / skew / picket spacing) runs on one warp.
 #include "pf_common.cuh"
 
 namespace epid {
@@ -17,8 +17,9 @@ constexpr int FIN_WARPS = FIN_THREADS / 32;
 constexpr int FIN_LPL = (PF_L + 31) / 32;       // leaf slots per lane
 
 // np.median of n non-negative doubles a[0..n) (shared memory) by the whole block: radix selection of the lower middle order
-// statistic on the bit patterns (for non-negative doubles the unsigned order of the bits is the order of the values), eight 8-bit
-// digits, warp-aggregated shared-memory histograms; the upper middle value is the same value if it occurs often enough, else the
+// statistic on the bit patterns (for non-negative doubles the unsigned order of the bits is the order of the values), up to eight
+// 8-bit digits, warp-aggregated shared-memory histograms, stopping at the first digit whose bucket holds one value; the upper
+// middle value is the same value if it occurs often enough, else the
 // smallest larger one.  Thread 0 returns the median; every thread must call.
 __device__ inline double block_median_nonneg_f64(const double* __restrict__ a, int n) {
     __shared__ uint32_t s_hist[256];
@@ -55,7 +56,11 @@ __device__ inline double block_median_nonneg_f64(const double* __restrict__ a, i
             if (k >= cum && k < inc) {      // exactly one lane
 #pragma unroll
                 for (int e = 0; e < 8; e++) {
-                    if (k >= cum && k < cum + loc[e]) { s_k = k - cum; s_prefix = prefix | ((unsigned long long)(tid * 8 + e) << shift); }
+                    if (k >= cum && k < cum + loc[e]) {
+                        s_k = k - cum;
+                        s_prefix = prefix | ((unsigned long long)(tid * 8 + e) << shift);
+                        s_cle = loc[e];
+                    }
                     cum += loc[e];
                 }
             }
@@ -64,6 +69,16 @@ __device__ inline double block_median_nonneg_f64(const double* __restrict__ a, i
         prefix = s_prefix;
         k = s_k;
         mask |= 0xffull << shift;
+        if (s_cle == 1u) {      // one value has this prefix: it is the order statistic, the lower digits need no more rounds
+            __syncthreads();    // every thread has read s_prefix
+            for (int i = tid; i < n; i += FIN_THREADS) {
+                const unsigned long long kv = keyat(i);
+                if ((kv & mask) == prefix) s_prefix = kv;
+            }
+            __syncthreads();
+            prefix = s_prefix;
+            break;
+        }
     }
     // upper middle value
     if (tid == 0) { s_cle = 0; s_above = ~0ull; }
@@ -85,18 +100,21 @@ __device__ inline double block_median_nonneg_f64(const double* __restrict__ a, i
     return (n & 1) ? v1 : (v1 + v2) / 2.0;
 }
 
-__global__ void __launch_bounds__(FIN_THREADS)
+// 64 registers at 256 threads: four CTAs per SM, so a batch of up to 528 frames runs in one wave on 132 SMs
+__global__ void __launch_bounds__(FIN_THREADS, 4)
 k_pf_finalize(const PfConst* __restrict__ cc, PfFrame* fr, const PfWin* __restrict__ wins, epid_pf_summary* __restrict__ summ,
               epid_pf_meas* __restrict__ meas_all) {
     extern __shared__ double s_err[];                    // pow2(2 * meas_cap) doubles for the median of |errors|
-    __shared__ int s_cnt[PF_L], s_off[PF_L], s_keep[PF_L];
+    __shared__ int s_cnt[PF_L], s_off[PF_L], s_keep[PF_L], s_leafnum[PF_L];
     __shared__ uint32_t s_vmask[PF_L];
     __shared__ double s_upper[PF_L], s_centre[PF_L];
-    __shared__ double s_fit[PF_P][2];
+    __shared__ double s_fit[PF_P][2], s_offp[PF_P], s_srt[PF_P];
+    __shared__ double s_cax, s_xmid;
+    __shared__ int s_hist[PF_P + 1];                     // leaf rows per kiss count
     __shared__ int s_i[8];
     __shared__ double s_wbuf[FIN_WARPS][PF_L], s_wsort[FIN_WARPS][PF_L];
     __shared__ double s_rmax[FIN_WARPS];
-    __shared__ int s_rarg[FIN_WARPS], s_rpass[FIN_WARPS], s_rfail[FIN_WARPS];
+    __shared__ int s_rarg[FIN_WARPS], s_rloc[FIN_WARPS], s_rpass[FIN_WARPS], s_rfail[FIN_WARPS];
 
     const int fi = blockIdx.x;
     const PfConst& c = *cc;
@@ -106,6 +124,7 @@ k_pf_finalize(const PfConst* __restrict__ cc, PfFrame* fr, const PfWin* __restri
     const int H = c.H, W = c.W;
     // every word of the row is defined, whatever the frame's fate: rows of different runs / pipelines compare equal byte for byte
     for (int k = tid; k < (int)(sizeof(epid_pf_summary) / 4); k += FIN_THREADS) reinterpret_cast<uint32_t*>(&S)[k] = 0u;
+    if (tid <= PF_P) s_hist[tid] = 0;
     __syncthreads();
     if (tid == 0) {
         S.status = f.status;
@@ -118,6 +137,10 @@ k_pf_finalize(const PfConst* __restrict__ cc, PfFrame* fr, const PfWin* __restri
         S.n_meas = 0;
         S.n_leaves_removed = 0;
         S.picket_spacing_px = f.spacing;
+        // dist2cax (picketfence.py:1905-1923) / image.center (core/image.py:526-533, PFDicomImage.center :246-260)
+        const int orient = f.orientation;
+        s_cax = c.p.has_cax_override ? (orient == 0 ? c.p.cax_x_px : c.p.cax_y_px) : (orient == 0 ? (double)W : (double)H) / 2.0 - 0.5;
+        s_xmid = rint((double)(orient == 0 ? H : W) / 2.0);
     }
     if (tid < PF_P) {
         S.picket_idx[tid] = tid < f.n_pickets ? f.picket_idx[tid] : 0;
@@ -133,12 +156,15 @@ k_pf_finalize(const PfConst* __restrict__ cc, PfFrame* fr, const PfWin* __restri
     const double n_axis_half = (orient == 0 ? (double)H : (double)W) / 2.0;
     const double ratio = c.p.leaf_analysis_width_ratio;
     // ---- kisses per leaf row, marker-line geometry of the row (picketfence.py:1725-1743)
+    if (tid < np) s_offp[tid] = fmax((double)f.picket_idx[tid] - spacing / 2.0, 0.0);   // picketfence.py:1618-1627
     for (int l = tid; l < nl; l += FIN_THREADS) {
         uint32_t m = 0;
         for (int p = 0; p < np; p++) m |= (wf[l * PF_P + p].valid ? 1u : 0u) << p;
         s_vmask[l] = m;
         s_cnt[l] = __popc(m);
+        if (m) atomicAdd(&s_hist[__popc(m)], 1);
         const int leaf = f.inview[l];
+        s_leafnum[l] = c.p.leaf_num[leaf];
         const double lw_px = c.p.leaf_width_mm[leaf] * dpmm;
         const double lc_px = c.p.leaf_center_mm[leaf] * dpmm + n_axis_half;
         const double upper = lc_px - lw_px / 2.0 * ratio;
@@ -147,90 +173,76 @@ k_pf_finalize(const PfConst* __restrict__ cc, PfFrame* fr, const PfWin* __restri
         s_centre[l] = (lower - upper) / 2.0 + upper;          // Line.center (core/geometry.py:556-561)
     }
     __syncthreads();
-    if (tid == 0) {
-        // median over the leaf rows that have at least one measurement (group_by on mlc_meas, picketfence.py:810-814);
-        // counts are <= 32, so a counting sort gives the two middle order statistics
-        int hist[PF_P + 1];
-        for (int k = 0; k <= PF_P; k++) hist[k] = 0;
-        int ng = 0, total = 0;
-        for (int l = 0; l < nl; l++)
-            if (s_cnt[l] > 0) { hist[s_cnt[l]]++; ng++; total += s_cnt[l]; }
+    if (wid == 0) {
+        // median over the leaf rows that have at least one measurement (group_by on mlc_meas, picketfence.py:810-814): counts are
+        // 1..32, lane k - 1 holds the rows with k, and its inclusive scan locates the two middle order statistics
+        const int h = s_hist[lane + 1];
+        int acc = h;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const int t = __shfl_up_sync(0xffffffffu, acc, o);
+            if (lane >= o) acc += t;
+        }
+        const int ng = __shfl_sync(0xffffffffu, acc, 31);
+        const int total = warp_sum(h * (lane + 1));
         int status = EPID_PF_OK;
         int removed = 0;
         if (total == 0) {
             status = EPID_PF_NO_MEASUREMENTS;
         } else {
             const int ka = (ng & 1) ? ng / 2 : ng / 2 - 1, kb = ng / 2;
-            int va = 0, vb = 0, acc = 0;
-            bool ha = false, hb = false;
-            for (int k = 1; k <= PF_P; k++) {
-                acc += hist[k];
-                if (!ha && acc > ka) { va = k; ha = true; }
-                if (!hb && acc > kb) { vb = k; hb = true; }
-            }
+            const int va = __ffs(__ballot_sync(0xffffffffu, acc > ka)), vb = __ffs(__ballot_sync(0xffffffffu, acc > kb));
             const int med_twice = va + vb;                     // 2 * statistics.median
+            // keep flags, and each row's offset in the table: an exclusive scan of the kept rows' counts
             int off = 0;
-            for (int l = 0; l < nl; l++) {
-                const bool keep = s_cnt[l] > 0 && 2 * s_cnt[l] == med_twice;
-                s_keep[l] = keep ? 1 : 0;
-                s_off[l] = off;
-                if (keep) off += s_cnt[l];
-                else if (s_cnt[l] > 0) removed++;
+            for (int base = 0; base < nl; base += 32) {
+                const int l = base + lane;
+                const int cnt = l < nl ? s_cnt[l] : 0;
+                const bool keep = cnt > 0 && 2 * cnt == med_twice;
+                const int v = keep ? cnt : 0;
+                int inc = v;
+#pragma unroll
+                for (int o = 1; o < 32; o <<= 1) {
+                    const int t = __shfl_up_sync(0xffffffffu, inc, o);
+                    if (lane >= o) inc += t;
+                }
+                if (l < nl) { s_keep[l] = keep ? 1 : 0; s_off[l] = off + inc - v; }
+                off += __shfl_sync(0xffffffffu, inc, 31);
+                removed += __popc(__ballot_sync(0xffffffffu, cnt > 0 && !keep));
             }
             if (off == 0) status = EPID_PF_NO_MEASUREMENTS;     // a .5 median drops every row (reference: polyfit of nothing)
             else if (off > c.meas_cap) status = EPID_PF_CAPACITY;
             s_i[1] = off;
         }
-        s_i[0] = status;
-        S.n_leaves_removed = removed;
-        if (status != EPID_PF_OK) { S.status = status; f.status = status; }
+        if (lane == 0) {
+            s_i[0] = status;
+            S.n_leaves_removed = removed;
+            if (status != EPID_PF_OK) { S.status = status; f.status = status; }
+        }
     }
     __syncthreads();
     if (s_i[0] != EPID_PF_OK) return;
     const int M = s_i[1];
     epid_pf_meas* meas = meas_all + (size_t)fi * c.meas_cap;
-    // ---- measurement table, leaf-major / picket-minor (= PicketFence.mlc_meas order): thread per (leaf, picket)
     const int npairs = nl * np;
-    for (int t = tid; t < npairs; t += FIN_THREADS) {
-        const int l = t / np, p = t - l * np;
-        const uint32_t vm = s_vmask[l];
-        if (!s_keep[l] || !((vm >> p) & 1u)) continue;
-        const int q = s_off[l] + __popc(vm & ((1u << p) - 1u));
-        const PfWin w = wf[l * PF_P + p];
-        epid_pf_meas& m = meas[q];
-        m.leaf_num = c.p.leaf_num[f.inview[l]];
-        m.picket = p;
-        const double offp = fmax((double)f.picket_idx[p] - spacing / 2.0, 0.0);   // picketfence.py:1618-1627
-        if (npos == 2) {
-            m.position[0] = w.l + offp;
-            m.position[1] = w.r + offp;
-        } else {
-            m.position[0] = fabs(w.r - w.l) / 2.0 + w.l + offp;                       // center_idx (core/profile.py:322-327)
-            m.position[1] = 0.0;
-        }
-        m.width_mm = (fmax(w.r, w.l) - fmin(w.r, w.l)) / dpmm;                        // field_width_px / dpmm
-    }
-    // ---- per-picket line fit np.polyfit(along-leaf-stack, along-travel, 1)  (picketfence.py:1881-1899): warp per picket
+    // ---- per-picket line fit np.polyfit(along-leaf-stack, along-travel, 1)  (picketfence.py:1881-1899): warp per picket.
+    //      The second pass reloads the windows (L1 hits) instead of holding FIN_LPL slots of three doubles per lane.
     for (int p = wid; p < np; p += FIN_WARPS) {
-        const double offp = fmax((double)f.picket_idx[p] - spacing / 2.0, 0.0);
-        double xv[FIN_LPL], y0[FIN_LPL], y1[FIN_LPL];
-        bool on[FIN_LPL];
+        const double offp = s_offp[p];
+        uint32_t on = 0;
         double sx = 0, sy = 0;
         int n = 0;
 #pragma unroll
         for (int it = 0; it < FIN_LPL; it++) {
             const int l = it * 32 + lane;
-            on[it] = l < nl && s_keep[l] && ((s_vmask[l] >> p) & 1u);
-            xv[it] = 0; y0[it] = 0; y1[it] = 0;
-            if (on[it]) {
+            if (l < nl && s_keep[l] && ((s_vmask[l] >> p) & 1u)) {
+                on |= 1u << it;
                 const PfWin w = wf[l * PF_P + p];
-                xv[it] = s_upper[l];
+                const double xv = s_upper[l];
                 if (npos == 2) {
-                    y0[it] = w.l + offp; y1[it] = w.r + offp;
-                    sx += xv[it] * 2.0; sy += y0[it] + y1[it]; n += 2;
+                    sx += xv * 2.0; sy += (w.l + offp) + (w.r + offp); n += 2;
                 } else {
-                    y0[it] = fabs(w.r - w.l) / 2.0 + w.l + offp;
-                    sx += xv[it]; sy += y0[it]; n += 1;
+                    sx += xv; sy += fabs(w.r - w.l) / 2.0 + w.l + offp; n += 1;
                 }
             }
         }
@@ -245,10 +257,12 @@ k_pf_finalize(const PfConst* __restrict__ cc, PfFrame* fr, const PfWin* __restri
         double sxx = 0, sxy = 0;
 #pragma unroll
         for (int it = 0; it < FIN_LPL; it++) {
-            if (on[it]) {
-                const double dx = xv[it] - mx_;
-                if (npos == 2) { sxx += 2.0 * dx * dx; sxy += dx * (y0[it] - my_) + dx * (y1[it] - my_); }
-                else { sxx += dx * dx; sxy += dx * (y0[it] - my_); }
+            if ((on >> it) & 1u) {
+                const int l = it * 32 + lane;
+                const PfWin w = wf[l * PF_P + p];
+                const double dx = s_upper[l] - mx_;
+                if (npos == 2) { sxx += 2.0 * dx * dx; sxy += dx * ((w.l + offp) - my_) + dx * ((w.r + offp) - my_); }
+                else { sxx += dx * dx; sxy += dx * ((fabs(w.r - w.l) / 2.0 + w.l + offp) - my_); }
             }
         }
         sxx = warp_sum(sxx);
@@ -260,98 +274,133 @@ k_pf_finalize(const PfConst* __restrict__ cc, PfFrame* fr, const PfWin* __restri
         }
     }
     __syncthreads();
-    if (tid == 0) {
-        int bad = 0;
-        for (int p = 0; p < np; p++)
-            if (s_fit[p][0] != s_fit[p][0]) bad = 1;   // a picket without measurements: polyfit([]) raises
-        s_i[2] = bad;
-        if (bad) { S.status = 7; f.status = 7; }
-    }
-    __syncthreads();
-    if (s_i[2]) return;
-    // ---- errors (picketfence.py:1701-1718) + per-thread partial aggregates
+    const int bad = __syncthreads_or(tid < np && s_fit[tid][0] != s_fit[tid][0]);   // a picket without measurements: polyfit([]) raises
+    // ---- measurement table, leaf-major / picket-minor (= PicketFence.mlc_meas order), and its errors (picketfence.py:1701-1718):
+    //      thread per (leaf, picket), plus per-thread partial aggregates.  The table is written whatever the fits.
     int m2n = 1;
     while (m2n < M * npos) m2n <<= 1;
-    for (int q = M * npos + tid; q < m2n; q += FIN_THREADS) s_err[q] = __longlong_as_double(0x7ff0000000000000LL);
-    int t_pass = 0, t_failed = 0, t_arg = 0x7fffffff;
+    if (!bad)
+        for (int q = M * npos + tid; q < m2n; q += FIN_THREADS) s_err[q] = __longlong_as_double(0x7ff0000000000000LL);
+    int t_pass = 0, t_failed = 0, t_arg = 0x7fffffff, t_loc = 0;
     double t_max = -1.0;
+#pragma unroll 1
     for (int t = tid; t < npairs; t += FIN_THREADS) {
         const int l = t / np, p = t - l * np;
         const uint32_t vm = s_vmask[l];
         if (!s_keep[l] || !((vm >> p) & 1u)) continue;
         const int q = s_off[l] + __popc(vm & ((1u << p) - 1u));
+        const PfWin w = wf[l * PF_P + p];
         epid_pf_meas& m = meas[q];
-        const double fitv = s_fit[p][0] * s_centre[l] + s_fit[p][1];
-        double me = 0.0;
-        bool allp = true;
-        for (int s = 0; s < npos; s++) {
-            double picket_pos = fitv;
-            if (npos == 2) picket_pos += (s == 0 ? -1.0 : 1.0) * c.p.nominal_gap_mm / 2.0 * dpmm;
-            const double e = (m.position[s] - picket_pos) / dpmm;
-            const int ok = fabs(e) < c.p.tolerance ? 1 : 0;
-            m.error[s] = e;
-            m.passed[s] = ok;
-            s_err[q * npos + s] = fabs(e);
-            t_pass += ok;
-            if (!ok) allp = false;
-            me = fmax(me, fabs(e));
+        m.leaf_num = s_leafnum[l];
+        m.picket = p;
+        const double offp = s_offp[p];
+        double pos0, pos1;
+        if (npos == 2) {
+            pos0 = w.l + offp;
+            pos1 = w.r + offp;
+        } else {
+            pos0 = fabs(w.r - w.l) / 2.0 + w.l + offp;                       // center_idx (core/profile.py:322-327)
+            pos1 = 0.0;
         }
-        if (npos == 1) { m.error[1] = 0.0; m.passed[1] = 1; }
-        if (!allp) t_failed++;
-        if (me > t_max) { t_max = me; t_arg = q; }     // q grows with t: first maximum of this thread's subsequence
+        m.position[0] = pos0;
+        m.position[1] = pos1;
+        m.width_mm = (fmax(w.r, w.l) - fmin(w.r, w.l)) / dpmm;                // field_width_px / dpmm
+        if (bad) continue;
+        const double fitv = s_fit[p][0] * s_centre[l] + s_fit[p][1];
+        const double tol = c.p.tolerance;
+        double e0, e1 = 0.0;
+        int ok1 = 1;
+        if (npos == 2) {
+            const double half_gap = c.p.nominal_gap_mm / 2.0 * dpmm;     // the marker lines of the two banks: fit -+ half the gap
+            e0 = (pos0 - (fitv - half_gap)) / dpmm;
+            e1 = (pos1 - (fitv + half_gap)) / dpmm;
+            ok1 = fabs(e1) < tol ? 1 : 0;
+            s_err[2 * q] = fabs(e0);
+            s_err[2 * q + 1] = fabs(e1);
+        } else {
+            e0 = (pos0 - fitv) / dpmm;
+            s_err[q] = fabs(e0);
+        }
+        const int ok0 = fabs(e0) < tol ? 1 : 0;
+        m.error[0] = e0;
+        m.error[1] = e1;
+        m.passed[0] = ok0;
+        m.passed[1] = ok1;
+        t_pass += ok0 + (npos == 2 ? ok1 : 0);
+        if (!(ok0 && ok1)) t_failed++;
+        const double me = fmax(fmax(0.0, fabs(e0)), fabs(e1));
+        if (me > t_max) {              // q grows with t: first maximum of this thread's subsequence, with its picket, row and bank
+            t_max = me;
+            t_arg = q;
+            t_loc = (npos == 2 && !(fabs(e0) > fabs(e1)) ? 1 : 0) | (p << 1) | (l << 6);
+        }
+    }
+    if (bad) {
+        if (tid == 0) { S.status = 7; f.status = 7; }
+        return;
     }
     // block reduction; first maximum in table order = stable descending sort .first()
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
         const double om = __shfl_xor_sync(0xffffffffu, t_max, o);
-        const int oa = __shfl_xor_sync(0xffffffffu, t_arg, o);
-        if (om > t_max || (om == t_max && oa < t_arg)) { t_max = om; t_arg = oa; }
+        const int oa = __shfl_xor_sync(0xffffffffu, t_arg, o), ol = __shfl_xor_sync(0xffffffffu, t_loc, o);
+        if (om > t_max || (om == t_max && oa < t_arg)) { t_max = om; t_arg = oa; t_loc = ol; }
     }
     t_pass = warp_sum(t_pass);
     t_failed = warp_sum(t_failed);
-    if (lane == 0) { s_rmax[wid] = t_max; s_rarg[wid] = t_arg; s_rpass[wid] = t_pass; s_rfail[wid] = t_failed; }
+    if (lane == 0) { s_rmax[wid] = t_max; s_rarg[wid] = t_arg; s_rloc[wid] = t_loc; s_rpass[wid] = t_pass; s_rfail[wid] = t_failed; }
     __syncthreads();
-    // ---- aggregates
-    if (tid == 0) {
-        int n_pass = 0, n_failed = 0, arg = s_rarg[0];
-        double max_err = s_rmax[0];
-        for (int k = 0; k < FIN_WARPS; k++) {
-            n_pass += s_rpass[k];
-            n_failed += s_rfail[k];
-            if (s_rmax[k] > max_err || (s_rmax[k] == max_err && s_rarg[k] < arg)) { max_err = s_rmax[k]; arg = s_rarg[k]; }
+    // ---- aggregates: warp 0, lane per picket
+    if (wid == 0) {
+        double max_err = lane < FIN_WARPS ? s_rmax[lane] : -2.0;
+        int arg = lane < FIN_WARPS ? s_rarg[lane] : 0x7fffffff, loc = lane < FIN_WARPS ? s_rloc[lane] : 0;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const double om = __shfl_xor_sync(0xffffffffu, max_err, o);
+            const int oa = __shfl_xor_sync(0xffffffffu, arg, o), ol = __shfl_xor_sync(0xffffffffu, loc, o);
+            if (om > max_err || (om == max_err && oa < arg)) { max_err = om; arg = oa; loc = ol; }
         }
-        const int n_tot = M * npos;
-        S.n_meas = M;
-        S.percent_passing = 100.0 * (double)n_pass / (double)n_tot;
-        S.max_error_mm = max_err;
-        S.max_error_picket = meas[arg].picket;
-        S.max_error_leaf = meas[arg].leaf_num;
-        S.max_error_bank = (npos == 2 && !(fabs(meas[arg].error[0]) > fabs(meas[arg].error[1]))) ? 1 : 0;
-        S.passed = n_pass == n_tot ? 1 : 0;
-        S.n_failed = n_failed;
-        // dist2cax (picketfence.py:1905-1923) / image.center (core/image.py:526-533, PFDicomImage.center :246-260)
-        double cax;
-        if (c.p.has_cax_override) cax = orient == 0 ? c.p.cax_x_px : c.p.cax_y_px;
-        else cax = (orient == 0 ? (double)W : (double)H) / 2.0 - 0.5;
-        S.cax_px = cax;
-        const int length = orient == 0 ? H : W;
-        const double xmid = rint((double)length / 2.0);
-        double d2c[PF_P], srt[PF_P];
+        const int n_pass = warp_sum(lane < FIN_WARPS ? s_rpass[lane] : 0);
+        const int n_failed = warp_sum(lane < FIN_WARPS ? s_rfail[lane] : 0);
+        const double cax = s_cax, xmid = s_xmid;
+        double d2c = 0.0, deg = 0.0;
+        if (lane < np) {
+            const double slope = s_fit[lane][0], icpt = s_fit[lane][1];
+            S.fit_slope[lane] = slope;
+            S.fit_intercept[lane] = icpt;
+            d2c = (cax - (slope * xmid + icpt)) / dpmm;
+            S.offsets_from_cax_mm[lane] = d2c;
+            deg = slope * (180.0 / 3.14159265358979323846);
+        }
+        // stable rank of the offset (a NaN offset, from a NaN cax override, ranks after the numbers), and the sums in picket order
+        const bool nan_me = d2c != d2c;
+        int rank = 0;
         double skew = 0.0;
         for (int p = 0; p < np; p++) {
-            S.fit_slope[p] = s_fit[p][0];
-            S.fit_intercept[p] = s_fit[p][1];
-            d2c[p] = (cax - (s_fit[p][0] * xmid + s_fit[p][1])) / dpmm;
-            S.offsets_from_cax_mm[p] = d2c[p];
-            skew += s_fit[p][0] * (180.0 / 3.14159265358979323846);
-            int j = p;
-            while (j > 0 && srt[j - 1] > d2c[p]) { srt[j] = srt[j - 1]; j--; }
-            srt[j] = d2c[p];
+            const double o = __shfl_sync(0xffffffffu, d2c, p);
+            skew += __shfl_sync(0xffffffffu, deg, p);
+            const bool nan_o = o != o;
+            rank += (nan_me ? (!nan_o || p < lane) : (!nan_o && (o < d2c || (o == d2c && p < lane)))) ? 1 : 0;
         }
-        S.mlc_skew = skew / (double)np;
+        if (lane < np) s_srt[rank] = d2c;
+        __syncwarp();
+        const double gap = lane + 1 < np ? fabs(s_srt[lane] - s_srt[lane + 1]) : 0.0;
         double sp = 0.0;
-        for (int p = 0; p + 1 < np; p++) sp += fabs(srt[p] - srt[p + 1]);
-        S.mean_picket_spacing_mm = np > 1 ? sp / (double)(np - 1) : __longlong_as_double(0x7ff8000000000000LL);
+        for (int p = 0; p + 1 < np; p++) sp += __shfl_sync(0xffffffffu, gap, p);
+        if (lane == 0) {
+            const int n_tot = s_i[1] * npos;
+            S.n_meas = s_i[1];
+            S.percent_passing = 100.0 * (double)n_pass / (double)n_tot;
+            S.max_error_mm = max_err;
+            S.max_error_picket = (loc >> 1) & (PF_P - 1);
+            S.max_error_leaf = s_leafnum[loc >> 6];
+            S.max_error_bank = loc & 1;
+            S.passed = n_pass == n_tot ? 1 : 0;
+            S.n_failed = n_failed;
+            S.cax_px = cax;
+            S.mlc_skew = skew / (double)np;
+            S.mean_picket_spacing_mm = np > 1 ? sp / (double)(np - 1) : __longlong_as_double(0x7ff8000000000000LL);
+        }
     }
     // ---- picket widths (picketfence.py:471-491): warp per picket, rank sort of <= 160 widths in shared memory
     for (int p = wid; p < np; p += FIN_WARPS) {
