@@ -160,7 +160,11 @@ enum { /* per-frame status (maps to the reference's exceptions) */
     EPID_PF_TOO_MANY_PICKETS = 3,  /* more than EPID_PF_MAX_PICKETS peaks (unsupported) */
     EPID_PF_WINDOW_NO_PEAK = 4,    /* reference would raise IndexError inside FWXMProfile.field_edge_idx */
     EPID_PF_CAPACITY = 5,          /* measurement table capacity exceeded */
-    EPID_PF_FLAT_IMAGE = 6         /* max == min: the reference divides by zero */
+    EPID_PF_FLAT_IMAGE = 6,        /* max == min: the reference divides by zero */
+    EPID_PF_EMPTY_FIT = 7,         /* a picket keeps no measurement, or a .5 median kiss count keeps no leaf row: the reference's
+                                      np.polyfit of nothing raises TypeError (picketfence.py:810-828, 1881-1899) */
+    EPID_PF_NAN_SPACING = 8        /* one picket and no picket_spacing: np.median(np.diff([i])) is nan and the reference raises
+                                      ValueError "cannot convert float NaN to integer" in _get_mlc_window (picketfence.py:869-886) */
 };
 
 typedef struct {

@@ -250,6 +250,8 @@ def pf_analyze(frame, dpmm, *, crop_mm=3, filter=None, mlc="Millennium", toleran
         by_leaf.setdefault(m["leaf"], []).append(m)
     median_n = statistics.median([len(v) for v in by_leaf.values()])
     full = [k for k, v in by_leaf.items() if len(v) == median_n]
+    # the reference keeps no count of the dropped rows: leaf rows with a measurement minus the rows kept
+    out["n_leaves_removed"] = len(by_leaf) - len(full)
     meas = [m for m in meas if m["leaf"] in full]
     out["n_meas"] = len(meas)
 

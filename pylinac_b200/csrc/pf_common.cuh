@@ -413,6 +413,7 @@ __device__ inline void pf_profile_block(const PfConst& c, PfFrame& f, const uint
                 }
             }
             f.spacing = spacing;
+            if (spacing != spacing) f.status = EPID_PF_NAN_SPACING;        // no window has bounds: int(nan) raises
             // _leaves_in_view (picketfence.py:888-912)
             const double n_axis = (double)(orient == 0 ? H : W);
             const double ratio = c.p.leaf_analysis_width_ratio;

@@ -210,7 +210,7 @@ k_pf_finalize(const PfConst* __restrict__ cc, PfFrame* fr, const PfWin* __restri
                 off += __shfl_sync(0xffffffffu, inc, 31);
                 removed += __popc(__ballot_sync(0xffffffffu, cnt > 0 && !keep));
             }
-            if (off == 0) status = EPID_PF_NO_MEASUREMENTS;     // a .5 median drops every row (reference: polyfit of nothing)
+            if (off == 0) status = EPID_PF_EMPTY_FIT;           // a .5 median drops every row (reference: polyfit of nothing)
             else if (off > c.meas_cap) status = EPID_PF_CAPACITY;
             s_i[1] = off;
         }
@@ -336,7 +336,7 @@ k_pf_finalize(const PfConst* __restrict__ cc, PfFrame* fr, const PfWin* __restri
         }
     }
     if (bad) {
-        if (tid == 0) { S.status = 7; f.status = 7; }
+        if (tid == 0) { S.status = EPID_PF_EMPTY_FIT; f.status = EPID_PF_EMPTY_FIT; }
         return;
     }
     // block reduction; first maximum in table order = stable descending sort .first()

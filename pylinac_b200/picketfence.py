@@ -106,6 +106,7 @@ STATUS_EXCEPTIONS = {
     5: (MemoryError, "Measurement table / window capacity exceeded."),
     6: (ValueError, "The image is flat (max == min); cannot normalize."),
     7: (TypeError, "expected non-empty vector for x (a picket has no MLC measurements)."),
+    8: (ValueError, "cannot convert float NaN to integer (one picket was found, so the picket spacing is nan: pass picket_spacing)."),
 }
 
 

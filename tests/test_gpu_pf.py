@@ -2,6 +2,7 @@
 
 Bars (BASELINE.json north_star): bit-exact for orientation, picket indices, leaf / picket / kiss counts, pass flags;
 <= 0.01 px for sub-pixel positions (we assert 1e-6 px; the fp64 profile arithmetic mirrors scipy's operation order)."""
+import builtins
 import warnings
 
 import numpy as np
@@ -30,9 +31,12 @@ def gpu_run(name):
 
 def _compare_with_golden(r, name, GOLD):
     if f"{name}/raises" in GOLD:
+        # goldens that record the reference's exception type hold it in raises_type; the older ones only raised ValueError
+        exc = getattr(builtins, str(GOLD[f"{name}/raises_type"])) if f"{name}/raises_type" in GOLD else ValueError
         assert r.status != 0
-        with pytest.raises(ValueError):
+        with pytest.raises(exc) as ei:
             r.raise_for_status()
+        assert type(ei.value) is exc, (r.status, ei.value)
         return
     assert r.status == 0, r.status
     g = lambda k: GOLD[f"{name}/{k}"]

@@ -54,11 +54,14 @@ def test_pf_random_case_matches_oracle(seed):
         warnings.simplefilter("ignore")
         try:
             o = pf_oracle.pf_analyze(a, dpmm, **ck, **ak)
-        except ValueError:
-            o = None
+        except (ValueError, TypeError, IndexError) as e:
+            o = e
     r = pf.analyze_batch(a[None], dpmm, **ck, **ak)[0]
-    if o is None:
+    if isinstance(o, Exception):
         assert r.status != 0
+        with pytest.raises(type(o)) as ei:
+            r.raise_for_status()
+        assert type(ei.value) is type(o), (r.status, o)
         return
     assert r.status == 0, (r.status, ck, ak)
     assert int(r.s["orientation"]) == int(o["orientation"])
@@ -71,3 +74,24 @@ def test_pf_random_case_matches_oracle(seed):
     assert bool(r.s["passed"]) == bool(o["passed"])
     np.testing.assert_allclose(float(r.s["max_error_mm"]), float(o["max_error"]), rtol=0, atol=ERR_TOL_MM)
     np.testing.assert_allclose(float(r.s["percent_passing"]), float(o["percent_passing"]), rtol=0, atol=1e-9)
+    # everything else the oracle returns: the front end's decisions, the fits and the per-picket aggregates
+    s = r.s
+    npk = int(s["n_pickets"])
+    assert npk == o["number_of_pickets"]
+    assert int(s["noise_median_passes"]) == o["noise_median_passes"]
+    assert bool(s["corner_inverted"]) == o["corner_inverted"]
+    assert (int(s["height"]), int(s["width"])) == tuple(o["shape"])
+    assert int(s["n_leaves_removed"]) == o["n_leaves_removed"]
+    np.testing.assert_array_equal(s["picket_spacing_px"], o["picket_spacing"])
+    np.testing.assert_allclose(r.m["width_mm"], o["meas_width_mm"], rtol=0, atol=ERR_TOL_MM)
+    np.testing.assert_allclose(s["fit_slope"][:npk], o["fits"][:, 0], rtol=0, atol=1e-9)
+    np.testing.assert_allclose(s["fit_intercept"][:npk], o["fits"][:, 1], rtol=0, atol=POS_TOL_PX)
+    np.testing.assert_allclose(s["offsets_from_cax_mm"][:npk], o["offsets_from_cax_mm"], rtol=0, atol=ERR_TOL_MM)
+    np.testing.assert_allclose(float(s["cax_px"]) / dpmm, o["cax_mm"], rtol=0, atol=1e-12)
+    for key, ok in [("abs_median_error_mm", "abs_median_error"), ("mean_picket_spacing_mm", "mean_picket_spacing"), ("mlc_skew", "mlc_skew")]:
+        np.testing.assert_allclose(float(s[key]), float(o[ok]), rtol=0, atol=ERR_TOL_MM, err_msg=key)
+    pw = np.stack([s["picket_width_max"][:npk], s["picket_width_mean"][:npk], s["picket_width_median"][:npk], s["picket_width_min"][:npk]], axis=1)
+    np.testing.assert_allclose(pw, o["picket_widths"], rtol=0, atol=ERR_TOL_MM)
+    assert int(s["max_error_picket"]) == o["max_error_picket"]
+    assert str(r.max_error_leaf) == str(o["max_error_leaf"])
+    assert [str(x) for x in r.failed_leaves()] == [str(x) for x in o["failed_leaves"]]
