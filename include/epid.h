@@ -668,6 +668,53 @@ int32_t epid_gamma_stats(epid_ctx* ctx, const epid_batch* gamma, double* sum, in
 int32_t epid_stack_mip(epid_ctx* ctx, const epid_batch* volume, epid_batch** colmax, epid_batch** rowmax);
 int32_t epid_cbct_views(epid_ctx* ctx, const epid_batch* z0, const epid_batch* z1, int32_t src_dtype, epid_batch** out);
 
+/* ----------------------------------------------------------------------------------------- light / radiation field coincidence
+ * StandardImagingFC2 and its subclasses (IMTLRad, DoselabRLf, IsoAlign, SNCFSQA; planar_imaging.py:1169-1727) and
+ * QuasarLightRadScaling (contrib/quasar.py:1-66) for a batch of uint16 frames, one result per frame:
+ *   ImagePhantomBase.__init__ ground / normalize (:226-231), check_inversion (core/image.py:868-897), invert, _find_field_info
+ *   (strip means -> FWXMProfilePhysical(ground, BEAM_CENTER)), _determine_bb_set, _detect_bb_centers (median filter, near-edge
+ *   equalize_adapthist + median filter, SizedDiskLocator.from_center_physical per BB), Quasar's _detect_scaling_centers.
+ * The set of nominal BB positions comes from the host (bb_mm: nbb (x, y) pairs; bb15_mm: the 15x15 set of set_mode 1).  Averages,
+ * offsets and the SNC FSQA virtual centre are host arithmetic on the returned points. */
+#define EPID_LR_MAX_BB 5
+#define EPID_LR_SCALING 5
+enum {
+    EPID_LR_OK = 0,
+    EPID_LR_NO_FIELD = 1,     /* no FWXM peak in a strip profile: IndexError in FWXMProfile.field_edge_idx */
+    EPID_LR_MISMATCH = 2,     /* x and y field widths differ by more than 10 mm (FC-2 set selection): ValueError */
+    EPID_LR_NO_BB = 3,        /* a BB window (or the Quasar scaling window) holds fewer disks than required: ValueError */
+    EPID_LR_CAPACITY = 4      /* a search window or region larger than the locator's shared-memory tiles */
+};
+enum { EPID_LR_SET_FIXED = 0, EPID_LR_SET_FC2 = 1, EPID_LR_SET_QUASAR = 2 };
+typedef struct {
+    double dpmm;
+    double fwxm;                       /* percent */
+    double bb_edge_threshold_mm;
+    double bb_size_mm, bb_box_mm, strip_width_mm;
+    double quasar_offset_mm;           /* set_mode EPID_LR_SET_QUASAR: BBs this far inside the field corners */
+    double bb_mm[2 * EPID_LR_MAX_BB], bb15_mm[2 * EPID_LR_MAX_BB];
+    int32_t nbb, set_mode;
+    int32_t normalize, invert;
+    int32_t clahe_kernel;              /* int(round(bb_size_mm / 2 * dpmm * kernel_size_multiplier)) */
+    int32_t scaling;                   /* Quasar: locate the 5 scaling BBs in a 35 mm window about the image centre */
+} epid_lr_params;
+
+typedef struct { /* one per frame */
+    int32_t status;
+    int32_t inverted;                  /* check_inversion fired (before the `invert` argument is applied) */
+    int32_t large_set;                 /* set_mode EPID_LR_SET_FC2: the 15x15 positions were used */
+    int32_t near_edge_mask;            /* bit k: BB k was located on the equalised (CLAHE) image */
+    int32_t failed_bb;                 /* EPID_LR_NO_BB: index of the first BB that was not found (nbb: the scaling search) */
+    int32_t n_found;                   /* disks found in that window */
+    int32_t n_scaling;
+    int32_t pad;
+    double field_center_x, field_center_y, field_width_x_mm, field_width_y_mm;
+    double bb_x[EPID_LR_MAX_BB], bb_y[EPID_LR_MAX_BB];
+    double scaling_x[EPID_LR_SCALING], scaling_y[EPID_LR_SCALING];
+} epid_lr_result;
+
+int32_t epid_lightrad_analyze(epid_ctx* ctx, const epid_batch* frames, const epid_lr_params* p, epid_lr_result* results);
+
 /* ----------------------------------------------------------------------------------------- multi-GPU (NCCL)
  * The batch shards by frame index with no data-path collective; the only exchange is the final gather of the
  * fixed-size per-frame result structs (SURVEY.md 8e).  id: 128-byte ncclUniqueId created by rank 0. */

@@ -248,6 +248,27 @@ VMAT_RESULT_DTYPE = np.dtype([
 
 
 
+LR_MAX_BB = 5
+LR_SCALING = 5
+
+
+class LrParams(C.Structure):
+    """epid_lr_params (include/epid.h)"""
+
+    _fields_ = [("dpmm", C.c_double), ("fwxm", C.c_double), ("bb_edge_threshold_mm", C.c_double), ("bb_size_mm", C.c_double),
+                ("bb_box_mm", C.c_double), ("strip_width_mm", C.c_double), ("quasar_offset_mm", C.c_double),
+                ("bb_mm", C.c_double * (2 * LR_MAX_BB)), ("bb15_mm", C.c_double * (2 * LR_MAX_BB)), ("nbb", C.c_int32),
+                ("set_mode", C.c_int32), ("normalize", C.c_int32), ("invert", C.c_int32), ("clahe_kernel", C.c_int32),
+                ("scaling", C.c_int32)]
+
+
+LR_RESULT_DTYPE = np.dtype([
+    ("status", "<i4"), ("inverted", "<i4"), ("large_set", "<i4"), ("near_edge_mask", "<i4"), ("failed_bb", "<i4"), ("n_found", "<i4"),
+    ("n_scaling", "<i4"), ("pad_", "<i4"), ("field_center_x", "<f8"), ("field_center_y", "<f8"), ("field_width_x_mm", "<f8"),
+    ("field_width_y_mm", "<f8"), ("bb_x", "<f8", (LR_MAX_BB,)), ("bb_y", "<f8", (LR_MAX_BB,)), ("scaling_x", "<f8", (LR_SCALING,)),
+    ("scaling_y", "<f8", (LR_SCALING,))], align=True)
+
+
 class LocateParams(C.Structure):
     _fields_ = [("mode", C.c_int32), ("invert", C.c_int32), ("sample_kind", C.c_int32), ("conditions", C.c_int32), ("dpmm", C.c_double),
                 ("radius_mm", C.c_double), ("tolerance_mm", C.c_double), ("field_width_mm", C.c_double), ("field_height_mm", C.c_double),
@@ -318,6 +339,7 @@ _SIGNATURES = {
     "epid_divide": [_P, _P, _P, _P, C.POINTER(_P)],
     "epid_dlg_analyze": [_P, _P, C.c_int32, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P],
     "epid_global_locate": [_P, _P, C.POINTER(LocateParams), _P, C.c_int32, _P, _P],
+    "epid_lightrad_analyze": [_P, _P, C.POINTER(LrParams), _P],
     "epid_canny": [_P, _P, _P, C.c_int32, C.c_double, C.c_double, C.POINTER(_P)],
     "epid_hough_line": [_P, _P, C.c_int32, _P, C.POINTER(_P), C.POINTER(C.c_int32)],
     "epid_hough_candidates": [_P, _P, C.c_int32, C.c_int32, C.c_double, C.c_int32, _P, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
@@ -888,6 +910,19 @@ def vmat_analyze(ctx: Context, img1, img2, params: VmatParams) -> np.ndarray:
             b1.free()
         if own2:
             b2.free()
+    return res
+
+
+def lightrad_analyze(ctx: Context, frames, params: LrParams) -> np.ndarray:
+    """Light / radiation field coincidence on uint16 frames (Batch or ndarray [n,h,w] / [h,w]) -> one LR_RESULT_DTYPE row per frame."""
+    b, own = _as_batch(ctx, frames, (np.dtype(np.uint16),))
+    (n, _, _), _ = b.shape_dtype
+    res = np.zeros(n, LR_RESULT_DTYPE)
+    try:
+        check(lib().epid_lightrad_analyze(ctx.handle, b.handle, C.byref(params), _ptr(res)))
+    finally:
+        if own:
+            b.free()
     return res
 
 

@@ -22,12 +22,12 @@
 #include "common.cuh"
 #include "peaks.cuh"
 #include "roi.cuh"
+#include "profile1d.cuh"
 
 namespace epid {
 
 constexpr int VM_ROWS = 64;          // rows per CTA of the front kernel
 constexpr int VM_THREADS = 256;
-#define VM_INF (__longlong_as_double(0x7ff0000000000000LL))
 
 struct VmAcc { unsigned int mn, mx; unsigned long long sum; };
 
@@ -141,27 +141,6 @@ __global__ void k_vmat_front_v16(const uint16_t* __restrict__ a, const uint16_t*
 }
 
 // ------------------------------------------------------------------------------------------------ block helpers (fp64)
-struct OpMin { __device__ static double f(double a, double b) { return fmin(a, b); } };
-struct OpMax { __device__ static double f(double a, double b) { return fmax(a, b); } };
-struct OpSum { __device__ static double f(double a, double b) { return a + b; } };
-
-template <class Op>
-__device__ double blk_reduce(double v, double* red) {      // red: >= 33 doubles of shared memory; result broadcast to every thread
-    const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = (blockDim.x + 31) >> 5;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = Op::f(v, __shfl_xor_sync(0xffffffffu, v, o));
-    __syncthreads();
-    if (lane == 0) red[wid] = v;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        double t = red[0];
-        for (int k = 1; k < nw; k++) t = Op::f(t, red[k]);
-        red[32] = t;
-    }
-    __syncthreads();
-    return red[32];
-}
-
 // image state: processed pixel = sign * v + off, with its current min / max
 struct VmMap { int sign; long long off; long long mn, mx; };
 
@@ -206,31 +185,6 @@ struct VmWork {          // per-pair global work area
     double* vals;        // [W]
     PeakWork pw;
 };
-
-// FWXMProfile.field_edge_idx: find_peaks(values, fwxm_height=0.5, max_number=1) -> left / right interpolated positions
-__device__ inline int vm_edges(const double* v, int n, PeakWork& pw, double* l, double* r) {
-    PeakArgs a;
-    a.hmin = -VM_INF;
-    a.distance = 1;
-    a.pmin = -1.0;
-    a.wmin = 0.0;
-    a.rel_height = 1.0 - 0.5;
-    a.max_number = 1;
-    a.sort_by_height = 0;
-    const int c = block_find_peaks(v, n, a, pw);
-    __syncthreads();
-    if (c < 1) return 2;
-    *l = pw.lip[0];
-    *r = pw.rip[0];
-    return 0;
-}
-
-__device__ inline double vm_lerp_at(const double* v, int n, double x) {      // UnivariateSpline(k=1, s=0) through (i, v[i])
-    int i = (int)floor(x);
-    i = max(0, min(i, n - 2));
-    const double u = x - (double)i;
-    return v[i] * (1.0 - u) + v[i + 1] * u;
-}
 
 // Order statistics k and k2 (= k or k + 1) of n values that are all >= +0 (no NaN): 8-bit radix select on the IEEE bit patterns (8 passes of
 // a 256-bin shared-memory histogram over the values that share the prefix found so far), then the successor: the same value when it

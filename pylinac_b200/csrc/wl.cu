@@ -31,6 +31,7 @@
 
 #include "pf_common.cuh"
 #include "ccl.cuh"
+#include "wl.cuh"
 
 namespace epid {
 
@@ -390,7 +391,8 @@ __device__ __forceinline__ void wl_union(int* parent, int a, int b) {
 __global__ void __launch_bounds__(WL_THREADS)
 k_wl_bb(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, const WlFrame* __restrict__ wf, double* __restrict__ samples,
         unsigned short* __restrict__ cid_all, WlComp* __restrict__ comp_all, epid_wl_result* __restrict__ res,
-        epid_disk_result* __restrict__ dres) {
+        epid_disk_result* __restrict__ dres, const uint16_t* const* __restrict__ item_src = nullptr,
+        const epid_disk_params* __restrict__ item_loc = nullptr) {
     extern __shared__ __align__(16) unsigned char smraw[];
     __shared__ int s_i[16];
     __shared__ int s_added;
@@ -402,6 +404,8 @@ k_wl_bb(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, const
     const int fi = blockIdx.x, tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
     const WlFrame F = wf[fi];
     const bool loc = c.loc_mode != 0;
+    // locator items (launch_disk_items): block = item, each with its own source frame and search parameters
+    const epid_disk_params& L = item_loc ? item_loc[fi] : c.loc;
     epid_wl_result r_unused;
     epid_wl_result& R = loc ? r_unused : res[fi];      // the locator reports through dres
     if (loc && tid == 0) { dres[fi].status = F.status; dres[fi].n_points = 0; dres[fi].n_regions = 0; dres[fi].passes = 0; }
@@ -416,13 +420,13 @@ k_wl_bb(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, const
     }
     if (F.status != EPID_WL_OK) return;
     const int H = c.H, W = c.W;
-    const uint16_t* f = base + (size_t)fi * H * W;
+    const uint16_t* f = item_src ? item_src[fi] : base + (size_t)fi * H * W;
     const int h = F.h, w = F.w, crop = F.crop;
     const double dpmm = c.p.dpmm, Dd = (double)F.D;
     // ---- SizedDiskLocator.from_center_physical((0, 0), window 40 + bb) (metrics/image.py:564-612)
-    const double bb_d = loc ? 2 * c.loc.radius_mm : c.p.bb_size_mm;
-    const double winx = loc ? c.loc.window_w : (40 + bb_d) * dpmm, winy = loc ? c.loc.window_h : (40 + bb_d) * dpmm;
-    const double ex = loc ? c.loc.expected_x : (double)w / 2, ey = loc ? c.loc.expected_y : (double)h / 2;
+    const double bb_d = loc ? 2 * L.radius_mm : c.p.bb_size_mm;
+    const double winx = loc ? L.window_w : (40 + bb_d) * dpmm, winy = loc ? L.window_h : (40 + bb_d) * dpmm;
+    const double ex = loc ? L.expected_x : (double)w / 2, ey = loc ? L.expected_y : (double)h / 2;
     // metrics/image.py:583-591: floor / ceil bounds, the slice clips at the image edge
     const int left = min(max((int)floor(ex - winx / 2), 0), w), right = max(min((int)ceil(ex + winx / 2), w), 0);
     const int top = min(max((int)floor(ey - winy / 2), 0), h), bottom = max(min((int)ceil(ey + winy / 2), h), 0);
@@ -457,7 +461,7 @@ k_wl_bb(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, const
     __syncthreads();
     if (gmin == gmax) { if (tid == 0) { R.status = EPID_WL_NO_BB; if (loc) dres[fi].status = EPID_WL_NO_BB; } return; }     // stretch divides by zero, nothing is found
     const double amin = (double)gmin / Dd, amax = (double)gmax / Dd;
-    const bool inv = loc ? (c.loc.invert != 0) : !c.p.low_density_bb;
+    const bool inv = loc ? (L.invert != 0) : !c.p.low_density_bb;
     // invert: b = -a + max + min (decreasing); stretch: (b - bmin) / (bmax - bmin) * 1, then ground with value 0
     const double bmin = inv ? (-amax + amax) + amin : amin, bmax = inv ? (-amin + amax) + amin : amax;
     const double cmax = bmax - bmin;
@@ -475,15 +479,15 @@ k_wl_bb(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, const
     const double radius_mm = bb_d / 2;
     // _calculate_bb_tolerance: np.interp(bb_diameter, (1.5, 30), (2, 4)) (winston_lutz.py:1062-1067)
     double tol;
-    if (loc) tol = c.loc.tolerance_mm;
+    if (loc) tol = L.tolerance_mm;
     else if (bb_d <= 1.5) tol = 2.0;
     else if (bb_d >= 30.0) tol = 4.0;
     else { const double slope = (4.0 - 2.0) / (30.0 - 1.5); tol = slope * (bb_d - 1.5) + 2.0; }
     // detection conditions (metrics/features.py): all five for Winston-Lutz, the caller's subset for the stand-alone locator
-    const int cm = loc ? c.loc.conditions : 31;
+    const int cm = loc ? L.conditions : 31;
     const bool c_size = cm & 1, c_round = cm & 2, c_circ = cm & 4, c_sym = cm & 8, c_solid = cm & 16, c_modest = cm & 32;
-    const int max_number = loc ? min(max(c.loc.max_number, 1), WL_MAXPTS) : 1;
-    const double min_sep = loc ? c.loc.min_separation_px : 5.0 * dpmm;      // deduplicate_points_and_boundaries (metrics/utils.py:14-37)
+    const int max_number = loc ? min(max(L.max_number, 1), WL_MAXPTS) : 1;
+    const double min_sep = loc ? L.min_separation_px : 5.0 * dpmm;      // deduplicate_points_and_boundaries (metrics/utils.py:14-37)
     const double PI = 3.141592653589793;
     const double larger_area = PI * ((radius_mm + tol) * (radius_mm + tol));
     const double smaller_area = fmax(PI * ((radius_mm - tol) * (radius_mm - tol)), 2.0);
@@ -892,6 +896,59 @@ __global__ void k_loc_init(WlFrame* wf, int n, int H, int W) {
     f.h = H; f.w = W;
     f.mn = 0; f.D = 1;
     wf[i] = f;
+}
+}  // namespace epid
+
+namespace epid {
+__global__ void k_loc_items_init(const WlItemMap* __restrict__ maps, WlFrame* wf, int n, int H, int W) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    WlFrame f;
+    memset(&f, 0, sizeof(f));
+    f.status = maps[i].status;
+    f.h = H; f.w = W;
+    f.mn = maps[i].mn; f.D = maps[i].D;
+    wf[i] = f;
+}
+
+static size_t disk_items_layout(int n, size_t* o_cst, size_t* o_fr, size_t* o_smp, size_t* o_cid, size_t* o_cmp) {
+    size_t o = 0;
+    auto sz = [&](size_t b) { const size_t r = o; o += (b + 255) / 256 * 256; return r; };
+    *o_cst = sz(sizeof(WlConst)); *o_fr = sz(sizeof(WlFrame) * n);
+    *o_smp = sz(sizeof(double) * (size_t)n * WL_MAXWIN * WL_MAXWIN);
+    *o_cid = sz(sizeof(unsigned short) * (size_t)n * WL_MAXWIN * WL_MAXWIN); *o_cmp = sz(sizeof(WlComp) * (size_t)n);
+    return o;
+}
+
+size_t disk_items_scratch_bytes(int n_items) {
+    size_t a, b, c, d, e;
+    return disk_items_layout(n_items, &a, &b, &c, &d, &e);
+}
+
+int launch_disk_items(epid_ctx* ctx, cudaStream_t st, void* scratch, int n, int H, int W, double dpmm, double max_window_px,
+                      const uint16_t* const* d_src, const WlItemMap* d_maps, const epid_disk_params* d_loc, epid_disk_result* d_res) {
+    size_t o_cst, o_fr, o_smp, o_cid, o_cmp;
+    disk_items_layout(n, &o_cst, &o_fr, &o_smp, &o_cid, &o_cmp);
+    char* base = (char*)scratch;
+    WlConst hc;
+    memset(&hc, 0, sizeof(hc));
+    hc.p.dpmm = dpmm;
+    hc.H = H;
+    hc.W = W;
+    hc.loc_mode = 1;
+    int win_edge = (int)ceil(max_window_px) + 2;
+    if (win_edge > WL_MAXWIN) win_edge = WL_MAXWIN;      // larger windows report EPID_WL_CAPACITY per item
+    if (win_edge < 8) win_edge = 8;
+    hc.win_edge = win_edge;
+    const size_t bb_smem = sizeof(int) * (size_t)win_edge * win_edge + 2 * WL_TILE * WL_TILE + 64;
+    EPID_CUDA(cudaMemcpyAsync(base + o_cst, &hc, sizeof(hc), cudaMemcpyHostToDevice, st));
+    EPID_SMEM_OPT_IN(ctx, k_wl_bb, sizeof(int) * WL_MAXWIN * WL_MAXWIN + 2 * WL_TILE * WL_TILE + 64);
+    k_loc_items_init<<<(n + 127) / 128, 128, 0, st>>>(d_maps, (WlFrame*)(base + o_fr), n, H, W);
+    k_wl_bb<<<n, WL_THREADS, bb_smem, st>>>((const WlConst*)(base + o_cst), nullptr, (const WlFrame*)(base + o_fr), (double*)(base + o_smp),
+                                           (unsigned short*)(base + o_cid), (WlComp*)(base + o_cmp), nullptr, d_res, d_src, d_loc);
+    ctx->launches += 2;
+    EPID_CUDA(cudaGetLastError());
+    return EPID_OK;
 }
 }  // namespace epid
 
