@@ -715,6 +715,16 @@ typedef struct { /* one per frame */
 
 int32_t epid_lightrad_analyze(epid_ctx* ctx, const epid_batch* frames, const epid_lr_params* p, epid_lr_result* results);
 
+/* Diagnostic read-back of the light / rad stages: the launch sequence of epid_lightrad_analyze (same results), and per frame the
+ * host uint16 [n][h][w] planes of the first 3 x 3 median of the mapped frame (filtered), the equalize_adapthist output before the
+ * second median (equalised) and the second median (equalised_filtered), plus EPID_LR_INFO int64 values per frame in the order
+ * mn, mx, sum, corner, checked, inv, near_mask, fmn, fmx, umin, umax (raw range, raw frame sum, raw sum of the four corner boxes,
+ * check_inversion, final inversion, near-edge mask, range of the filtered frame, range of the equalised frame).  For frames with
+ * near_mask == 0 the equalised planes and fmn .. umax are unspecified. */
+#define EPID_LR_INFO 11
+int32_t epid_lightrad_stages(epid_ctx* ctx, const epid_batch* frames, const epid_lr_params* p, epid_lr_result* results,
+                             uint16_t* filtered, uint16_t* equalised, uint16_t* equalised_filtered, int64_t* info);
+
 /* ----------------------------------------------------------------------------------------- multi-GPU (NCCL)
  * The batch shards by frame index with no data-path collective; the only exchange is the final gather of the
  * fixed-size per-frame result structs (SURVEY.md 8e).  id: 128-byte ncclUniqueId created by rank 0. */

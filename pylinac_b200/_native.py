@@ -340,6 +340,7 @@ _SIGNATURES = {
     "epid_dlg_analyze": [_P, _P, C.c_int32, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P],
     "epid_global_locate": [_P, _P, C.POINTER(LocateParams), _P, C.c_int32, _P, _P],
     "epid_lightrad_analyze": [_P, _P, C.POINTER(LrParams), _P],
+    "epid_lightrad_stages": [_P, _P, C.POINTER(LrParams), _P, _P, _P, _P, _P],
     "epid_canny": [_P, _P, _P, C.c_int32, C.c_double, C.c_double, C.POINTER(_P)],
     "epid_hough_line": [_P, _P, C.c_int32, _P, C.POINTER(_P), C.POINTER(C.c_int32)],
     "epid_hough_candidates": [_P, _P, C.c_int32, C.c_int32, C.c_double, C.c_int32, _P, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
@@ -924,6 +925,27 @@ def lightrad_analyze(ctx: Context, frames, params: LrParams) -> np.ndarray:
         if own:
             b.free()
     return res
+
+
+LR_INFO_FIELDS = ("mn", "mx", "sum", "corner", "checked", "inv", "near_mask", "fmn", "fmx", "umin", "umax")
+
+
+def lightrad_stages(ctx: Context, frames, params: LrParams) -> dict:
+    """Diagnostic read-back of epid_lightrad_stages: {"results": LR_RESULT_DTYPE rows, "filtered", "equalised", "equalised_filtered":
+    uint16 [n, h, w], "info": {name: int64 [n]} for the names of LR_INFO_FIELDS}.  The equalised planes and fmn .. umax of frames
+    without a near-edge BB are unspecified."""
+    b, own = _as_batch(ctx, frames, (np.dtype(np.uint16),))
+    (n, h, w), _ = b.shape_dtype
+    res = np.zeros(n, LR_RESULT_DTYPE)
+    planes = [np.empty((n, h, w), np.uint16) for _ in range(3)]
+    info = np.zeros((n, len(LR_INFO_FIELDS)), np.int64)
+    try:
+        check(lib().epid_lightrad_stages(ctx.handle, b.handle, C.byref(params), _ptr(res), *[_ptr(a) for a in planes], _ptr(info)))
+    finally:
+        if own:
+            b.free()
+    return {"results": res, "filtered": planes[0], "equalised": planes[1], "equalised_filtered": planes[2],
+            "info": {name: info[:, k] for k, name in enumerate(LR_INFO_FIELDS)}}
 
 
 def divide(ctx: Context, num, den, sign_off=None) -> np.ndarray:

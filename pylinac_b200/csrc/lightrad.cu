@@ -30,7 +30,9 @@
 //   k_lr_items        one locator item per BB (+ the Quasar scaling search): source frame, pixel map, window
 //   k_wl_bb           (wl.cu, launch_disk_items) the windowed disk locator per item
 //   k_lr_finalize     per frame: points into the result row, exceptions in the reference's order
+// epid_lightrad_stages runs the same sequence and also copies the three planes and the per-frame accumulators back, for the tests.
 #include <cmath>
+#include <vector>
 
 #include "common.cuh"
 #include "filters.cuh"
@@ -492,11 +494,20 @@ __global__ void k_lr_finalize(const LrConst* __restrict__ cc, const LrFrame* __r
     }
 }
 
+// host destinations of the diagnostic read-back (epid_lightrad_stages); epid_lightrad_analyze passes none
+struct LrTap {
+    uint16_t* filtered;
+    uint16_t* equalised;
+    uint16_t* equalised_filtered;
+    LrFrame* frames;
+};
+
 }  // namespace epid
 
 using namespace epid;
 
-extern "C" int32_t epid_lightrad_analyze(epid_ctx* ctx, const epid_batch* frames, const epid_lr_params* p, epid_lr_result* results) {
+static int32_t lightrad_run(epid_ctx* ctx, const epid_batch* frames, const epid_lr_params* p, epid_lr_result* results,
+                            const LrTap* tap) {
     EPID_REQUIRE(ctx && frames && p && results, EPID_ERR_INVALID, "NULL argument");
     EPID_REQUIRE(frames->dtype == EPID_U16, EPID_ERR_UNSUPPORTED, "light/rad frames must be uint16");
     EPID_REQUIRE(p->dpmm > 0 && p->bb_size_mm > 0 && p->bb_box_mm > 0 && p->strip_width_mm > 0, EPID_ERR_INVALID, "bad geometry");
@@ -600,8 +611,36 @@ extern "C" int32_t epid_lightrad_analyze(epid_ctx* ctx, const epid_batch* frames
         ctx->launches += 1;
         EPID_CUDA(cudaGetLastError());
         EPID_CUDA(cudaMemcpyAsync(results + c0, base + o_res, sizeof(epid_lr_result) * cn, cudaMemcpyDeviceToHost, st));
+        if (tap) {
+            // stream order: the copies finish before the next chunk reuses the planes
+            const size_t pb = sizeof(uint16_t) * npx * cn;
+            EPID_CUDA(cudaMemcpyAsync(tap->filtered + (size_t)c0 * npx, d_filt, pb, cudaMemcpyDeviceToHost, st));
+            EPID_CUDA(cudaMemcpyAsync(tap->equalised + (size_t)c0 * npx, d_eq, pb, cudaMemcpyDeviceToHost, st));
+            EPID_CUDA(cudaMemcpyAsync(tap->equalised_filtered + (size_t)c0 * npx, d_eqf, pb, cudaMemcpyDeviceToHost, st));
+            EPID_CUDA(cudaMemcpyAsync(tap->frames + c0, d_fr, sizeof(LrFrame) * cn, cudaMemcpyDeviceToHost, st));
+        }
     }
     cudaError_t e = cudaStreamSynchronize(st);
     if (e != cudaSuccess) { set_error("light/rad pipeline failed: %s", cudaGetErrorString(e)); return EPID_ERR_CUDA; }
+    return EPID_OK;
+}
+
+extern "C" int32_t epid_lightrad_analyze(epid_ctx* ctx, const epid_batch* frames, const epid_lr_params* p, epid_lr_result* results) {
+    return lightrad_run(ctx, frames, p, results, nullptr);
+}
+
+extern "C" int32_t epid_lightrad_stages(epid_ctx* ctx, const epid_batch* frames, const epid_lr_params* p, epid_lr_result* results,
+                                        uint16_t* filtered, uint16_t* equalised, uint16_t* equalised_filtered, int64_t* info) {
+    EPID_REQUIRE(frames && filtered && equalised && equalised_filtered && info, EPID_ERR_INVALID, "NULL argument");
+    std::vector<LrFrame> fr((size_t)(frames->n > 0 ? frames->n : 0));
+    const LrTap tap{filtered, equalised, equalised_filtered, fr.data()};
+    const int32_t rc = lightrad_run(ctx, frames, p, results, &tap);
+    if (rc != EPID_OK) return rc;
+    for (size_t i = 0; i < fr.size(); i++) {
+        const LrFrame& F = fr[i];
+        const int64_t row[EPID_LR_INFO] = {F.mn, F.mx, (int64_t)F.sum, (int64_t)F.corner, F.checked, F.inv, F.near_mask,
+                                           F.fmn, F.fmx, F.umin, F.umax};
+        memcpy(info + i * EPID_LR_INFO, row, sizeof(row));
+    }
     return EPID_OK;
 }

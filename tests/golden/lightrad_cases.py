@@ -43,16 +43,43 @@ _C = {
     "snc": ("SNCFSQA", (1280, 1280), 0.336, 150.6, 150.3, (0.3, 0.2), (0.2, 0.2), 4, [(40, -40)], 18, False, {}, {}),
     "quasar": ("QuasarLightRadScaling", (1280, 1280), 0.336, 150.3, 150.8, (0.2, -0.1), (0.0, 0.0), 5, None, 19, False, {}, {}),
 }
+
+
+def multiplier_for(k: int, bb_size_mm: float, pixel_mm: float) -> float:
+    """the kernel_size_multiplier that makes the reference's CLAHE kernel int(round(bb_radius_px * multiplier)) equal k"""
+    return k / (bb_size_mm / 2 / pixel_mm)
+
+
+def _k(k, pixel_mm, bb_size_mm=4):
+    return {"kernel_size_multiplier": multiplier_for(k, bb_size_mm, pixel_mm)}
+
+
+# kernel sizes and frame shapes beyond the default k = int(round(bb_radius_px * 2)) in {9, 10, 12}: clip limits above 1, kernels that
+# divide the frame, partial tiles of odd frames, and k = 1, where every contextual region is one pixel
+_C.update({
+    "fc2_k1": ("StandardImagingFC2", (1280, 1280), 0.336, 99.6, 99.4, (0.3, -0.2), (0.0, 0.0), 4, SI_10, 20, False, _k(1, 0.336), {}),
+    "fc2_k32": ("StandardImagingFC2", (1280, 1280), 0.336, 99.5, 99.7, (-0.2, 0.1), (0.1, -0.1), 4, SI_10, 21, False, _k(32, 0.336),
+                {}),
+    "fc2_k64": ("StandardImagingFC2", (1280, 1280), 0.336, 99.3, 99.6, (0.1, 0.3), (-0.1, 0.1), 4, SI_10, 22, False, _k(64, 0.336),
+                {}),
+    "fc2_k160": ("StandardImagingFC2", (1280, 1280), 0.336, 99.7, 99.5, (0.2, 0.2), (0.0, 0.1), 4, SI_10, 23, False, _k(160, 0.336),
+                 {}),
+    "fc2_1190_near": ("StandardImagingFC2", (1190, 1190), 0.336, 99.4, 99.6, (-0.3, 0.2), (0.1, 0.0), 4, SI_10, 24, False, {}, {}),
+    "fc2_odd_small": ("StandardImagingFC2", (241, 199), 0.6, 99.5, 99.3, (0.2, -0.3), (0.1, 0.2), 4, SI_10, 25, False, {}, {}),
+    "fc2_no_normalize_k64": ("StandardImagingFC2", (1280, 1280), 0.336, 99.6, 99.2, (0.1, -0.1), (0.0, 0.2), 4, SI_10, 26, False,
+                             _k(64, 0.336), {"normalize": False}),
+    "fc2_inverted_k48": ("StandardImagingFC2", (1280, 1280), 0.336, 99.4, 99.5, (-0.1, 0.2), (0.2, 0.0), 4, SI_10, 27, True,
+                         _k(48, 0.336), {}),
+})
 CASES = list(_C)
 
 
-def _bbs(name):
-    spec = _C[name]
-    if spec[0] == "QuasarLightRadScaling":
-        fx, fy = spec[3] / 2, spec[4] / 2
+def _bbs_for(cls, fwx, fwy, bbs):
+    if cls == "QuasarLightRadScaling":
+        fx, fy = fwx / 2, fwy / 2
         corners = [(-fx + 11, -fy + 11), (-fx + 11, fy - 11), (fx - 11, fy - 11), (fx - 11, -fy + 11)]
         return corners + QUASAR_SCALING
-    return spec[8]
+    return bbs
 
 
 def _erf_edge(x, lo, hi, sigma):
@@ -62,9 +89,16 @@ def _erf_edge(x, lo, hi, sigma):
     return 0.5 * (erf((x - lo) / s) - erf((x - hi) / s))
 
 
-def lightrad_case(name):
-    """-> dict(cls, frame uint16 [h, w], dpmm, ctor, analyze, truth) for one named case"""
-    cls, (h, w), ps, fwx, fwy, (fcx, fcy), (box, boy), bbd, _, seed, inverted, ak, ck = _C[name]
+def synth_frame(cls, shape, pixel_mm, field_mm, field_offset_mm=(0.0, 0.0), bb_offset_mm=(0.0, 0.0), bb_diameter_mm=4, bbs=SI_10,
+                seed=0, inverted=False):
+    """-> (frame uint16 [h, w], truth) for one synthetic light/rad frame: field_mm = (x, y) widths, bbs = nominal BB positions (mm)
+    (ignored for Quasar, whose corner BBs follow the field)"""
+    h, w = shape
+    ps = pixel_mm
+    fwx, fwy = field_mm
+    fcx, fcy = field_offset_mm
+    box, boy = bb_offset_mm
+    bbd = bb_diameter_mm
     rng = np.random.default_rng(1000 + seed)
     dpmm = 1.0 / ps
     # pixel coordinates of the image centre as the reference places the nominal BBs (shape / 2)
@@ -78,7 +112,7 @@ def lightrad_case(name):
     bb_px = []
     r = bbd / 2 * dpmm
     yy, xx = np.mgrid[0:h, 0:w]
-    for bx, by in _bbs(name):
+    for bx, by in _bbs_for(cls, fwx, fwy, bbs):
         x0, y0 = w / 2 + (bx + box) * dpmm, h / 2 + (by + boy) * dpmm
         x0 += rng.uniform(-0.3, 0.3)
         y0 += rng.uniform(-0.3, 0.3)
@@ -98,4 +132,11 @@ def lightrad_case(name):
         "field_center_px": np.array([cx, cy]),
         "bb_px": np.array(bb_px, dtype=np.float64).reshape(-1, 2),
     }
-    return {"cls": cls, "frame": frame, "dpmm": dpmm, "ctor": dict(ck), "analyze": dict(ak), "truth": truth}
+    return frame, truth
+
+
+def lightrad_case(name):
+    """-> dict(cls, frame uint16 [h, w], dpmm, ctor, analyze, truth) for one named case"""
+    cls, shape, ps, fwx, fwy, fc, bo, bbd, bbs, seed, inverted, ak, ck = _C[name]
+    frame, truth = synth_frame(cls, shape, ps, (fwx, fwy), fc, bo, bbd, bbs, seed, inverted)
+    return {"cls": cls, "frame": frame, "dpmm": 1.0 / ps, "ctor": dict(ck), "analyze": dict(ak), "truth": truth}

@@ -32,7 +32,7 @@ def test_lightrad_case_inputs_reproduce(name):
 
 
 @pytest.mark.skipif(not os.path.isdir(os.path.join(REFERENCE_ROOT, "pylinac")), reason="needs the reference source tree")
-@pytest.mark.parametrize("name", ["fc2_10_near", "fc2_mismatch", "quasar", "snc"])
+@pytest.mark.parametrize("name", ["fc2_10_near", "fc2_mismatch", "quasar", "snc", "fc2_k1", "fc2_k64", "fc2_odd_small"])
 def test_lightrad_golden_reproduces_from_reference(name):
     import warnings
 
