@@ -129,9 +129,13 @@ int32_t epid_sobel(epid_ctx* ctx, const epid_batch* in, int32_t axis, epid_batch
  * prominence, width=min_width, rel_height = 1 - fwxm_height) + search-region trimming + top-max_number selection.
  * values: host double[n].  Arguments follow the reference's python signature after _parse_peak_args has NOT yet
  * been applied (threshold in [0,1] is a ratio of the range, separation in [0,1] a ratio of len, region <= 1 ratios).
- * peak_sort: 0 = 'prominences', 1 = 'peak_heights'.  max_number <= 0: all.  required_prominence < 0: none.
+ * peak_sort: 0 = 'prominences', 1 = 'peak_heights'.  required_prominence < 0: none.  max_number: EPID_PEAKS_ALL keeps every
+ * peak (python None); any other value k keeps [:k] of the peaks in descending peak_sort order, as the reference slices: 0 keeps
+ * none, -k all but the k smallest.  Equal keys rank the right-most peak first.  fwxm_height > 1 is EPID_ERR_INVALID (scipy's
+ * negative rel_height).
  * Outputs (capacity cap each): idx int64; heights, prominences, left_bases(int64), right_bases(int64), widths,
  * width_heights, left_ips, right_ips double.  *count = number of peaks returned. */
+#define EPID_PEAKS_ALL INT32_MIN
 typedef struct {
     double threshold;           /* -inf allowed */
     double peak_separation;

@@ -45,6 +45,9 @@ class NoDeviceError(NativeError):
     pass
 
 
+PEAKS_ALL = -(2 ** 31)   # EPID_PEAKS_ALL: max_number=None
+
+
 class PeakParams(C.Structure):
     _fields_ = [("threshold", C.c_double), ("peak_separation", C.c_double), ("max_number", C.c_int32),
                 ("fwxm_height", C.c_double), ("min_width", C.c_double), ("search_lo", C.c_double),
@@ -694,7 +697,7 @@ def find_peaks(ctx: Context, values, threshold=-np.inf, peak_separation=0, max_n
                search_region=(0.0, 1.0), peak_sort="prominences", required_prominence=None):
     v = np.ascontiguousarray(values, dtype=np.float64)
     n = v.size
-    p = PeakParams(float(threshold), float(peak_separation), int(max_number) if max_number else 0, float(fwxm_height),
+    p = PeakParams(float(threshold), float(peak_separation), PEAKS_ALL if max_number is None else int(max_number), float(fwxm_height),
                    float(min_width), float(search_region[0]), float(search_region[1]), 1 if peak_sort == "peak_heights" else 0,
                    -1.0 if required_prominence is None else float(required_prominence))
     cap = n // 2 + 2

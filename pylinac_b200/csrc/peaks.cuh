@@ -3,11 +3,15 @@
 // Reproduces, stage for stage, what pylinac.core.profile.find_peaks (core/profile.py:2545-2623) obtains from
 // scipy.signal.find_peaks(x, height, distance, prominence, width, rel_height)   (scipy/signal/_peak_finding.py:
 // _local_maxima_1d, _select_by_peak_distance, _peak_prominences, _peak_widths; restated in SURVEY.md appendix B):
-//   local maxima (plateau midpoint) -> height >= hmin -> distance (highest first; among equal heights the
-//   right-most survives) -> prominences (wlen=None) -> prominence >= pmin -> widths at rel_height -> width >= wmin
-//   -> keep the max_number largest by `peak_sort`, returned left to right.
-// All arithmetic is IEEE fp64 in the same operation order as the reference, so indices are bit-exact and the
-// interpolated positions agree to the last few ulps.
+//   local maxima (plateau midpoint) -> height >= hmin -> distance (highest first) -> prominences (wlen=None)
+//   -> prominence >= pmin -> widths at rel_height -> width >= wmin -> keep the max_number largest by `peak_sort`,
+//   returned left to right.
+// All arithmetic is IEEE fp64 in the same operation order as the reference (built with -fmad=false), so indices, bases,
+// prominences, width heights and interpolated positions are bit-exact.
+// Ties are resolved in one fixed order: among equal heights in the distance stage, and among equal keys at the
+// max_number cut, the right-most candidate ranks highest.  That is scipy's and the reference's result whenever
+// numpy's argsort keeps tied elements in their original order; the default argsort kind does not promise that, and
+// where it does not, the reference's result on tied inputs depends on the CPU it runs on.
 #pragma once
 #include "common.cuh"
 

@@ -33,6 +33,9 @@ extern "C" int32_t epid_find_peaks(epid_ctx* ctx, const double* values, int32_t 
                                    double* widths, double* width_heights, double* left_ips, double* right_ips, int32_t* count) {
     EPID_REQUIRE(ctx && values && p && count, EPID_ERR_INVALID, "NULL argument");
     EPID_REQUIRE(n >= 1, EPID_ERR_INVALID, "empty profile");
+    // scipy's _peak_widths rejects a negative rel_height before it looks at the peaks, so the reference raises for any profile
+    EPID_REQUIRE(!(1.0 - p->fwxm_height < 0.0), EPID_ERR_INVALID, "`rel_height` must be greater or equal to 0.0 (fwxm_height %g > 1)",
+                 p->fwxm_height);
     EPID_CUDA(cudaSetDevice(ctx->device));
     // ---- _parse_peak_args (core/profile.py:2626-2649) on the host: needs min/max of the values
     double vmin = values[0], vmax = values[0];
@@ -54,14 +57,17 @@ extern "C" int32_t epid_find_peaks(epid_ctx* ctx, const double* values, int32_t 
     if (hi < 0) hi += n; if (hi < 0) hi = 0; if (hi > n) hi = n;
     const int m = hi > lo ? hi - lo : 0;
     *count = 0;
-    if (m < 3) return EPID_OK;   // no interior sample -> no peak
+    if (m < 3 || p->max_number == 0) return EPID_OK;   // no interior sample -> no peak; [:0] keeps none
     PeakArgs a;
     a.hmin = thr;
     a.distance = (int)ceil(sep);
     a.pmin = p->required_prominence;
     a.wmin = p->min_width;
     a.rel_height = 1.0 - p->fwxm_height;
-    a.max_number = p->max_number;
+    // [:max_number] of the descending order: a negative max_number keeps all but the -max_number smallest, so a first launch
+    // counts the peaks and a second keeps count + max_number of them
+    const bool drop_smallest = p->max_number < 0 && p->max_number != EPID_PEAKS_ALL;
+    a.max_number = p->max_number > 0 ? p->max_number : 0;
     a.sort_by_height = p->peak_sort == 1;
     const int pcap = m / 2 + 1;
     int cap2 = 1;
@@ -89,12 +95,17 @@ extern "C" int32_t epid_find_peaks(epid_ctx* ctx, const double* values, int32_t 
         return epid_find_peaks(ctx, values, n, p, cap, idx, heights, prominences, left_bases, right_bases, widths, width_heights, left_ips, right_ips, count);
     }
     EPID_CUDA(cudaMemcpyAsync(d_x, values + lo, sizeof(double) * m, cudaMemcpyHostToDevice, ctx->stream));
-    k_find_peaks<<<1, FP_THREADS, 0, ctx->stream>>>(d_x, m, a, pcap, d_idx, d_prom, d_lb, d_rb, d_wh, d_lip, d_rip, d_flag, d_skey, d_sidx, d_out);
-    ctx->launches++;
     FpOut ho;
-    EPID_CUDA(cudaMemcpyAsync(&ho, d_out, sizeof(ho), cudaMemcpyDeviceToHost, ctx->stream));
-    EPID_CUDA(cudaStreamSynchronize(ctx->stream));
-    EPID_REQUIRE(ho.count >= 0, EPID_ERR_UNSUPPORTED, "peak capacity exceeded");
+    for (int pass = 0;; pass++) {
+        k_find_peaks<<<1, FP_THREADS, 0, ctx->stream>>>(d_x, m, a, pcap, d_idx, d_prom, d_lb, d_rb, d_wh, d_lip, d_rip, d_flag, d_skey, d_sidx, d_out);
+        ctx->launches++;
+        EPID_CUDA(cudaMemcpyAsync(&ho, d_out, sizeof(ho), cudaMemcpyDeviceToHost, ctx->stream));
+        EPID_CUDA(cudaStreamSynchronize(ctx->stream));
+        EPID_REQUIRE(ho.count >= 0, EPID_ERR_UNSUPPORTED, "peak capacity exceeded");
+        if (!drop_smallest || pass == 1) break;
+        a.max_number = ho.count + p->max_number;
+        if (a.max_number <= 0) return EPID_OK;
+    }
     const int c = ho.count;
     EPID_REQUIRE(c <= cap, EPID_ERR_INVALID, "output capacity %d too small for %d peaks", cap, c);
     std::vector<int> hi_idx(c), hlb(c), hrb(c);
