@@ -5,6 +5,7 @@ library is missing, or no CUDA device is visible, the compute entry points raise
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 import os
 import subprocess
@@ -65,25 +66,6 @@ class PFParams(C.Structure):
                 ("leaf_width_mm", C.c_double * PF_MAX_LEAVES), ("leaf_num", C.c_int32 * PF_MAX_LEAVES)]
 
 
-class PFSummary(C.Structure):
-    _fields_ = [("status", C.c_int32), ("orientation", C.c_int32), ("noise_median_passes", C.c_int32),
-                ("corner_inverted", C.c_int32), ("height", C.c_int32), ("width", C.c_int32), ("n_pickets", C.c_int32),
-                ("n_meas", C.c_int32), ("n_leaves_removed", C.c_int32), ("passed", C.c_int32),
-                ("max_error_picket", C.c_int32), ("max_error_leaf", C.c_int32), ("max_error_bank", C.c_int32),
-                ("n_failed", C.c_int32), ("picket_spacing_px", C.c_double), ("percent_passing", C.c_double),
-                ("max_error_mm", C.c_double), ("abs_median_error_mm", C.c_double), ("mean_picket_spacing_mm", C.c_double),
-                ("mlc_skew", C.c_double), ("cax_px", C.c_double), ("picket_idx", C.c_int32 * PF_MAX_PICKETS),
-                ("picket_val", C.c_double * PF_MAX_PICKETS), ("fit_slope", C.c_double * PF_MAX_PICKETS),
-                ("fit_intercept", C.c_double * PF_MAX_PICKETS), ("offsets_from_cax_mm", C.c_double * PF_MAX_PICKETS),
-                ("picket_width_max", C.c_double * PF_MAX_PICKETS), ("picket_width_mean", C.c_double * PF_MAX_PICKETS),
-                ("picket_width_median", C.c_double * PF_MAX_PICKETS), ("picket_width_min", C.c_double * PF_MAX_PICKETS)]
-
-
-class PFMeas(C.Structure):
-    _fields_ = [("leaf_num", C.c_int32), ("picket", C.c_int32), ("passed", C.c_int32 * 2), ("position", C.c_double * 2),
-                ("error", C.c_double * 2), ("width_mm", C.c_double)]
-
-
 PF_SUMMARY_DTYPE = np.dtype([
     ("status", "<i4"), ("orientation", "<i4"), ("noise_median_passes", "<i4"), ("corner_inverted", "<i4"),
     ("height", "<i4"), ("width", "<i4"), ("n_pickets", "<i4"), ("n_meas", "<i4"), ("n_leaves_removed", "<i4"),
@@ -97,8 +79,6 @@ PF_SUMMARY_DTYPE = np.dtype([
     ("picket_width_min", "<f8", (PF_MAX_PICKETS,))], align=True)
 PF_MEAS_DTYPE = np.dtype([("leaf_num", "<i4"), ("picket", "<i4"), ("passed", "<i4", (2,)), ("position", "<f8", (2,)),
                           ("error", "<f8", (2,)), ("width_mm", "<f8")], align=True)
-assert PF_SUMMARY_DTYPE.itemsize == C.sizeof(PFSummary), (PF_SUMMARY_DTYPE.itemsize, C.sizeof(PFSummary))
-assert PF_MEAS_DTYPE.itemsize == C.sizeof(PFMeas)
 
 STAR_MAX_PEAKS = 64
 
@@ -109,22 +89,13 @@ class StarParams(C.Structure):
                 ("fwhm", C.c_int32), ("recursive", C.c_int32), ("invert", C.c_int32)]
 
 
-class StarResult(C.Structure):
-    _fields_ = [("status", C.c_int32), ("hist_inverted", C.c_int32), ("start_x", C.c_int32), ("start_y", C.c_int32),
-                ("local_max", C.c_double), ("iterations", C.c_int32), ("profile_len", C.c_int32), ("radius_px", C.c_double),
-                ("n_peaks", C.c_int32), ("n_lines", C.c_int32), ("peak_idx", C.c_int32 * STAR_MAX_PEAKS),
-                ("peak_x", C.c_double * STAR_MAX_PEAKS), ("peak_y", C.c_double * STAR_MAX_PEAKS), ("wobble_x", C.c_double),
-                ("wobble_y", C.c_double), ("wobble_radius_px", C.c_double), ("wobble_radius_mm", C.c_double),
-                ("angles", C.c_double * (STAR_MAX_PEAKS // 2)), ("passed", C.c_int32), ("pad", C.c_int32)]
-
-
 STAR_RESULT_DTYPE = np.dtype([
     ("status", "<i4"), ("hist_inverted", "<i4"), ("start_x", "<i4"), ("start_y", "<i4"), ("local_max", "<f8"),
     ("iterations", "<i4"), ("profile_len", "<i4"), ("radius_px", "<f8"), ("n_peaks", "<i4"), ("n_lines", "<i4"),
     ("peak_idx", "<i4", (STAR_MAX_PEAKS,)), ("peak_x", "<f8", (STAR_MAX_PEAKS,)), ("peak_y", "<f8", (STAR_MAX_PEAKS,)),
     ("wobble_x", "<f8"), ("wobble_y", "<f8"), ("wobble_radius_px", "<f8"), ("wobble_radius_mm", "<f8"),
     ("angles", "<f8", (STAR_MAX_PEAKS // 2,)), ("passed", "<i4"), ("pad", "<i4")], align=True)
-assert STAR_RESULT_DTYPE.itemsize == C.sizeof(StarResult), (STAR_RESULT_DTYPE.itemsize, C.sizeof(StarResult))
+
 
 class FieldParams(C.Structure):
     _fields_ = [("dpmm", C.c_double), ("protocol", C.c_int32), ("centering", C.c_int32), ("vert_position", C.c_double),
@@ -135,8 +106,7 @@ class FieldParams(C.Structure):
                 ("edge", C.c_int32), ("edge_smoothing_ratio", C.c_double)]
 
 
-_FIELD_DOUBLES = ["top_penumbra_mm", "bottom_penumbra_mm", "left_penumbra_mm", "right_penumbra_mm"]
-_FIELD_LAYOUT = [
+FIELD_RESULT_DTYPE = np.dtype([
     ("status", "<i4"), ("hist_inverted", "<i4"), ("strip_rows", "<i4", (2,)), ("strip_cols", "<i4", (2,)), ("profile_len", "<i4", (2,)),
     ("top_penumbra_mm", "<f8"), ("bottom_penumbra_mm", "<f8"), ("left_penumbra_mm", "<f8"), ("right_penumbra_mm", "<f8"),
     ("geometric_center_index_x_y", "<f8", (2,)), ("beam_center_index_x_y", "<f8", (2,)),
@@ -148,20 +118,8 @@ _FIELD_LAYOUT = [
     ("top_horizontal_distance_from_beam_center_mm", "<f8"), ("top_vertical_distance_from_beam_center_mm", "<f8"),
     ("left_slope_percent_mm", "<f8"), ("right_slope_percent_mm", "<f8"), ("top_slope_percent_mm", "<f8"),
     ("bottom_slope_percent_mm", "<f8"), ("symmetry_horizontal", "<f8"), ("symmetry_vertical", "<f8"),
-    ("flatness_horizontal", "<f8"), ("flatness_vertical", "<f8")]
-FIELD_RESULT_DTYPE = np.dtype(_FIELD_LAYOUT, align=True)
+    ("flatness_horizontal", "<f8"), ("flatness_vertical", "<f8")], align=True)
 
-
-def _struct_from_layout(name, layout):
-    fields = []
-    for item in layout:
-        ct = C.c_int32 if item[1] == "<i4" else C.c_double
-        fields.append((item[0], ct * item[2][0] if len(item) == 3 else ct))
-    return type(name, (C.Structure,), {"_fields_": fields})
-
-
-FieldResult = _struct_from_layout("FieldResult", _FIELD_LAYOUT)
-assert FIELD_RESULT_DTYPE.itemsize == C.sizeof(FieldResult), (FIELD_RESULT_DTYPE.itemsize, C.sizeof(FieldResult))
 
 class SpParams(C.Structure):
     _fields_ = [("dpmm", C.c_double), ("interpolation", C.c_int32), ("interpolation_resolution_mm", C.c_double),
@@ -170,7 +128,7 @@ class SpParams(C.Structure):
                 ("edge_left", C.c_double), ("edge_right", C.c_double)]
 
 
-_SP_LAYOUT = [
+SP_RESULT_DTYPE = np.dtype([
     ("status", "<i4"), ("n", "<i4"), ("x_start", "<f8"), ("x_stop", "<f8"), ("values_max", "<f8"),
     ("geometric_center_index", "<f8"), ("geometric_center_value", "<f8"),
     ("beam_ok", "<i4"), ("fwxm_ok", "<i4"), ("infl_ok", "<i4"), ("pen_ok", "<i4"), ("fd_ok", "<i4"), ("fd_field_values_n", "<i4"),
@@ -184,8 +142,7 @@ _SP_LAYOUT = [
     ("fd_inner_left", "<f8"), ("fd_inner_right", "<f8"), ("fd_left_slope", "<f8"), ("fd_left_intercept", "<f8"),
     ("fd_right_slope", "<f8"), ("fd_right_intercept", "<f8"), ("fd_top_index", "<f8"), ("fd_top_value", "<f8"),
     ("fd_top_params", "<f8", (3,)), ("fd_beam_center_value", "<f8"), ("fd_cax_value", "<f8"), ("fd_left_value", "<f8"),
-    ("fd_right_value", "<f8")]
-SP_RESULT_DTYPE = np.dtype(_SP_LAYOUT, align=True)
+    ("fd_right_value", "<f8")], align=True)
 
 
 class WlParams(C.Structure):
@@ -194,13 +151,11 @@ class WlParams(C.Structure):
 
 
 (WL_OK, WL_NO_BB, WL_MISMATCH, WL_NO_FIELD, WL_CAPACITY, WL_FLAT_IMAGE) = range(6)
-_WL_LAYOUT = [
+WL_RESULT_DTYPE = np.dtype([
     ("status", "<i4"), ("inverted", "<i4"), ("crop_px", "<i4"), ("height", "<i4"), ("width", "<i4"), ("n_bbs", "<i4"),
     ("threshold_passes", "<i4"), ("pad", "<i4"), ("bb_x", "<f8"), ("bb_y", "<f8"), ("field_x", "<f8"), ("field_y", "<f8"),
     ("epid_x", "<f8"), ("epid_y", "<f8"), ("cax2bb_x", "<f8"), ("cax2bb_y", "<f8"), ("cax2bb_distance", "<f8"),
-    ("cax2epid_x", "<f8"), ("cax2epid_y", "<f8"), ("cax2epid_distance", "<f8")]
-WL_RESULT_DTYPE = np.dtype(_WL_LAYOUT, align=True)
-assert WL_RESULT_DTYPE.itemsize == 128
+    ("cax2epid_x", "<f8"), ("cax2epid_y", "<f8"), ("cax2epid_distance", "<f8")], align=True)
 DISK_MAX = 8
 
 
@@ -212,14 +167,12 @@ class DiskParams(C.Structure):
                 ("invert", C.c_int32), ("max_number", C.c_int32), ("conditions", C.c_int32), ("pad", C.c_int32)]
 
 
-DISK_RESULT_DTYPE = np.dtype([("status", np.int32), ("n_points", np.int32), ("n_regions", np.int32), ("passes", np.int32),
-                              ("left", np.int32), ("top", np.int32), ("x", np.float64, DISK_MAX), ("y", np.float64, DISK_MAX),
-                              ("r_area", np.float64, DISK_MAX), ("r_filled_area", np.float64, DISK_MAX),
-                              ("r_perimeter", np.float64, DISK_MAX), ("r_convex_area", np.float64, DISK_MAX),
-                              ("r_centroid_y", np.float64, DISK_MAX), ("r_centroid_x", np.float64, DISK_MAX),
-                              ("r_wcentroid_y", np.float64, DISK_MAX), ("r_wcentroid_x", np.float64, DISK_MAX),
-                              ("r_bbox", np.int32, (DISK_MAX, 4))], align=True)
-assert DISK_RESULT_DTYPE.itemsize == 24 + 8 * DISK_MAX * 10 + 4 * DISK_MAX * 4
+_D = (DISK_MAX,)
+DISK_RESULT_DTYPE = np.dtype([
+    ("status", "<i4"), ("n_points", "<i4"), ("n_regions", "<i4"), ("passes", "<i4"), ("left", "<i4"), ("top", "<i4"), ("x", "<f8", _D),
+    ("y", "<f8", _D), ("r_area", "<f8", _D), ("r_filled_area", "<f8", _D), ("r_perimeter", "<f8", _D), ("r_convex_area", "<f8", _D),
+    ("r_centroid_y", "<f8", _D), ("r_centroid_x", "<f8", _D), ("r_wcentroid_y", "<f8", _D), ("r_wcentroid_x", "<f8", _D),
+    ("r_bbox", "<i4", (DISK_MAX, 4))], align=True)
 _lib = None
 _lock = threading.Lock()
 
@@ -267,7 +220,7 @@ class LrParams(C.Structure):
 
 LR_RESULT_DTYPE = np.dtype([
     ("status", "<i4"), ("inverted", "<i4"), ("large_set", "<i4"), ("near_edge_mask", "<i4"), ("failed_bb", "<i4"), ("n_found", "<i4"),
-    ("n_scaling", "<i4"), ("pad_", "<i4"), ("field_center_x", "<f8"), ("field_center_y", "<f8"), ("field_width_x_mm", "<f8"),
+    ("n_scaling", "<i4"), ("pad", "<i4"), ("field_center_x", "<f8"), ("field_center_y", "<f8"), ("field_width_x_mm", "<f8"),
     ("field_width_y_mm", "<f8"), ("bb_x", "<f8", (LR_MAX_BB,)), ("bb_y", "<f8", (LR_MAX_BB,)), ("scaling_x", "<f8", (LR_SCALING,)),
     ("scaling_y", "<f8", (LR_SCALING,))], align=True)
 
@@ -509,6 +462,12 @@ class Batch:
             lib().epid_batch_free(self.handle)
             self.handle = None
 
+    def __enter__(self) -> "Batch":
+        return self
+
+    def __exit__(self, *exc) -> None:
+        self.free()
+
     def __del__(self):
         try:
             self.free()
@@ -524,6 +483,22 @@ class Batch:
         h = _P()
         check(fn(self.ctx.handle, self.handle, *args, C.byref(h)))
         return Batch(self.ctx, h)
+
+
+@contextlib.contextmanager
+def batch_for(ctx: Context, frames, dtype=None):
+    """The Batch `frames`, or the ndarray `frames` ([n, h, w] or [h, w]) uploaded for the block and freed after it.  An ndarray
+    that is not of `dtype` (when given) raises TypeError before anything reaches the device."""
+    if isinstance(frames, Batch):
+        yield frames
+        return
+    a = np.ascontiguousarray(frames)
+    if a.ndim == 2:
+        a = a[None]
+    if dtype is not None and a.dtype != dtype:
+        raise TypeError(f"{a.dtype} frames are not supported here; expected {np.dtype(dtype)}")
+    with Batch.upload(ctx, a) as b:
+        yield b
 
 
 def pinned_empty(shape, dtype=np.uint16) -> np.ndarray:
@@ -784,22 +759,13 @@ def gaussian_kernel_table(max_sigma: int):
 
 def starshot_analyze(ctx: Context, frames, params: StarParams) -> np.ndarray:
     """frames: a Batch (device-resident, uint16) or a uint16 ndarray [n,h,w] / [h,w]; one STAR_RESULT_DTYPE row per frame."""
-    own = None
-    if not isinstance(frames, Batch):
-        a = np.asarray(frames)
-        if a.dtype != np.uint16:
-            raise TypeError("starshot frames must be uint16")
-        own = frames = Batch.upload(ctx, a)
-    (n, h, w), _ = frames.shape_dtype
-    # CollapsedCircleProfile length <= 2 pi * 1.1 * 0.95 * (dim / 2) * 3; sigma = round(0.003 * length)
-    max_sigma = max(int(round(0.003 * (10 * max(h, w) + 64))) + 1, 2)
-    gw, go = gaussian_kernel_table(max_sigma)
-    res = np.zeros(n, STAR_RESULT_DTYPE)
-    try:
-        check(lib().epid_starshot_analyze(ctx.handle, frames.handle, C.byref(params), _ptr(gw), _ptr(go), max_sigma, _ptr(res)))
-    finally:
-        if own is not None:
-            own.free()
+    with batch_for(ctx, frames, np.uint16) as b:
+        (n, h, w), _ = b.shape_dtype
+        # CollapsedCircleProfile length <= 2 pi * 1.1 * 0.95 * (dim / 2) * 3; sigma = round(0.003 * length)
+        max_sigma = max(int(round(0.003 * (10 * max(h, w) + 64))) + 1, 2)
+        gw, go = gaussian_kernel_table(max_sigma)
+        res = np.zeros(n, STAR_RESULT_DTYPE)
+        check(lib().epid_starshot_analyze(ctx.handle, b.handle, C.byref(params), _ptr(gw), _ptr(go), max_sigma, _ptr(res)))
     return res
 
 
@@ -814,119 +780,65 @@ def gaussian_kernel1d(sigma: float, truncate: float = 4.0):
 
 def field_analyze(ctx: Context, frames, params: FieldParams) -> np.ndarray:
     """frames: a Batch (device-resident, uint16) or a uint16 ndarray [n,h,w] / [h,w]; one FIELD_RESULT_DTYPE row per frame."""
-    own = None
-    if not isinstance(frames, Batch):
-        a = np.asarray(frames)
-        if a.dtype != np.uint16:
-            raise TypeError("field analysis frames must be uint16")
-        own = frames = Batch.upload(ctx, a)
-    (n, h, w), _ = frames.shape_dtype
-    gh = gv = None
-    lh = lv = 0
-    if params.edge != 0:
-        # gaussian_filter1d(values, sigma=edge_smoothing_ratio * len(values)) (core/profile.py:1655-1659): one table per profile length
-        nh = lib().epid_field_profile_len(w, params.dpmm, params.interpolation, params.interpolation_resolution_mm)
-        nv = lib().epid_field_profile_len(h, params.dpmm, params.interpolation, params.interpolation_resolution_mm)
-        gh, lh = gaussian_kernel1d(params.edge_smoothing_ratio * nh)
-        gv, lv = gaussian_kernel1d(params.edge_smoothing_ratio * nv)
-    res = np.zeros(n, FIELD_RESULT_DTYPE)
-    try:
-        check(lib().epid_field_analyze(ctx.handle, frames.handle, C.byref(params), _ptr(gh), lh, _ptr(gv), lv, _ptr(res)))
-    finally:
-        if own is not None:
-            own.free()
+    with batch_for(ctx, frames, np.uint16) as b:
+        (n, h, w), _ = b.shape_dtype
+        gh = gv = None
+        lh = lv = 0
+        if params.edge != 0:
+            # gaussian_filter1d(values, sigma=edge_smoothing_ratio * len(values)) (core/profile.py:1655-1659): one table per profile length
+            nh = lib().epid_field_profile_len(w, params.dpmm, params.interpolation, params.interpolation_resolution_mm)
+            nv = lib().epid_field_profile_len(h, params.dpmm, params.interpolation, params.interpolation_resolution_mm)
+            gh, lh = gaussian_kernel1d(params.edge_smoothing_ratio * nh)
+            gv, lv = gaussian_kernel1d(params.edge_smoothing_ratio * nv)
+        res = np.zeros(n, FIELD_RESULT_DTYPE)
+        check(lib().epid_field_analyze(ctx.handle, b.handle, C.byref(params), _ptr(gh), lh, _ptr(gv), lv, _ptr(res)))
     return res
 
 
 def wl2d_analyze(ctx: Context, frames, params: WlParams) -> np.ndarray:
     """frames: a Batch (device-resident, uint16) or a uint16 ndarray [n,h,w] / [h,w]; one WL_RESULT_DTYPE row per frame."""
-    own = None
-    if not isinstance(frames, Batch):
-        a = np.asarray(frames)
-        if a.dtype != np.uint16:
-            raise TypeError("Winston-Lutz frames must be uint16")
-        own = frames = Batch.upload(ctx, a)
-    (n, _, _), _ = frames.shape_dtype
-    res = np.zeros(n, WL_RESULT_DTYPE)
-    try:
-        check(lib().epid_wl2d_analyze(ctx.handle, frames.handle, C.byref(params), _ptr(res)))
-    finally:
-        if own is not None:
-            own.free()
+    with batch_for(ctx, frames, np.uint16) as b:
+        (n, _, _), _ = b.shape_dtype
+        res = np.zeros(n, WL_RESULT_DTYPE)
+        check(lib().epid_wl2d_analyze(ctx.handle, b.handle, C.byref(params), _ptr(res)))
     return res
-
-
-def _as_batch(ctx: Context, frames, dtypes=None):
-    """-> (Batch, owned?) for a Batch or an ndarray [h,w] / [n,h,w]."""
-    if isinstance(frames, Batch):
-        return frames, False
-    a = np.ascontiguousarray(frames)
-    if a.ndim == 2:
-        a = a[None]
-    if dtypes is not None and a.dtype not in dtypes:
-        raise TypeError(f"dtype {a.dtype} is not supported here")
-    return Batch.upload(ctx, a), True
 
 
 def disk_locate(ctx: Context, frames, params: DiskParams) -> np.ndarray:
     """SizedDiskRegion / SizedDiskLocator on uint16 frames: one DISK_RESULT_DTYPE row per frame."""
-    b, own = _as_batch(ctx, frames, (np.dtype(np.uint16),))
-    (n, _, _), _ = b.shape_dtype
-    res = np.zeros(n, DISK_RESULT_DTYPE)
-    try:
+    with batch_for(ctx, frames, np.uint16) as b:
+        (n, _, _), _ = b.shape_dtype
+        res = np.zeros(n, DISK_RESULT_DTYPE)
         check(lib().epid_disk_locate(ctx.handle, b.handle, C.byref(params), _ptr(res)))
-    finally:
-        if own:
-            b.free()
     return res
 
 
 def roi_stats(ctx: Context, frames, verts_xy) -> dict:
     """RectangleROI statistics: verts_xy [nroi, 4, 2] corner (x, y) -> dict of [n, nroi] arrays (count, mean, std, min, max)."""
     v = np.ascontiguousarray(verts_xy, dtype=np.float64).reshape(-1, 4, 2)
-    b, own = _as_batch(ctx, frames)
-    (n, _, _), _ = b.shape_dtype
-    out = {k: np.empty((n, len(v))) for k in ("count", "mean", "std", "min", "max")}
-    try:
+    with batch_for(ctx, frames) as b:
+        (n, _, _), _ = b.shape_dtype
+        out = {k: np.empty((n, len(v))) for k in ("count", "mean", "std", "min", "max")}
         check(lib().epid_roi_stats(ctx.handle, b.handle, len(v), _ptr(v), _ptr(out["count"]), _ptr(out["mean"]), _ptr(out["std"]),
                                    _ptr(out["min"]), _ptr(out["max"])))
-    finally:
-        if own:
-            b.free()
     return out
 
 
 def vmat_analyze(ctx: Context, img1, img2, params: VmatParams) -> np.ndarray:
     """n (image 1, image 2) pairs of uint16 frames (Batch or ndarray [n,h,w] / [h,w]) -> one VMAT_RESULT_DTYPE row per pair."""
-    b1, own1 = _as_batch(ctx, img1, (np.dtype(np.uint16),))
-    try:
-        b2, own2 = _as_batch(ctx, img2, (np.dtype(np.uint16),))
-    except Exception:
-        if own1:
-            b1.free()
-        raise
-    (n, _, _), _ = b1.shape_dtype
-    res = np.zeros(n, VMAT_RESULT_DTYPE)
-    try:
+    with batch_for(ctx, img1, np.uint16) as b1, batch_for(ctx, img2, np.uint16) as b2:
+        (n, _, _), _ = b1.shape_dtype
+        res = np.zeros(n, VMAT_RESULT_DTYPE)
         check(lib().epid_vmat_analyze(ctx.handle, b1.handle, b2.handle, C.byref(params), _ptr(res)))
-    finally:
-        if own1:
-            b1.free()
-        if own2:
-            b2.free()
     return res
 
 
 def lightrad_analyze(ctx: Context, frames, params: LrParams) -> np.ndarray:
     """Light / radiation field coincidence on uint16 frames (Batch or ndarray [n,h,w] / [h,w]) -> one LR_RESULT_DTYPE row per frame."""
-    b, own = _as_batch(ctx, frames, (np.dtype(np.uint16),))
-    (n, _, _), _ = b.shape_dtype
-    res = np.zeros(n, LR_RESULT_DTYPE)
-    try:
+    with batch_for(ctx, frames, np.uint16) as b:
+        (n, _, _), _ = b.shape_dtype
+        res = np.zeros(n, LR_RESULT_DTYPE)
         check(lib().epid_lightrad_analyze(ctx.handle, b.handle, C.byref(params), _ptr(res)))
-    finally:
-        if own:
-            b.free()
     return res
 
 
@@ -937,16 +849,12 @@ def lightrad_stages(ctx: Context, frames, params: LrParams) -> dict:
     """Diagnostic read-back of epid_lightrad_stages: {"results": LR_RESULT_DTYPE rows, "filtered", "equalised", "equalised_filtered":
     uint16 [n, h, w], "info": {name: int64 [n]} for the names of LR_INFO_FIELDS}.  The equalised planes and fmn .. umax of frames
     without a near-edge BB are unspecified."""
-    b, own = _as_batch(ctx, frames, (np.dtype(np.uint16),))
-    (n, h, w), _ = b.shape_dtype
-    res = np.zeros(n, LR_RESULT_DTYPE)
-    planes = [np.empty((n, h, w), np.uint16) for _ in range(3)]
-    info = np.zeros((n, len(LR_INFO_FIELDS)), np.int64)
-    try:
+    with batch_for(ctx, frames, np.uint16) as b:
+        (n, h, w), _ = b.shape_dtype
+        res = np.zeros(n, LR_RESULT_DTYPE)
+        planes = [np.empty((n, h, w), np.uint16) for _ in range(3)]
+        info = np.zeros((n, len(LR_INFO_FIELDS)), np.int64)
         check(lib().epid_lightrad_stages(ctx.handle, b.handle, C.byref(params), _ptr(res), *[_ptr(a) for a in planes], _ptr(info)))
-    finally:
-        if own:
-            b.free()
     return {"results": res, "filtered": planes[0], "equalised": planes[1], "equalised_filtered": planes[2],
             "info": {name: info[:, k] for k, name in enumerate(LR_INFO_FIELDS)}}
 
@@ -957,51 +865,36 @@ def divide(ctx: Context, num, den, sign_off=None) -> np.ndarray:
     squeeze = a.ndim == 2
     if a.dtype != b.dtype or a.dtype not in (np.uint16, np.float64):
         a, b = a.astype(np.float64), b.astype(np.float64)
-    ba, bb = Batch.upload(ctx, a), Batch.upload(ctx, b)
     so = None if sign_off is None else np.ascontiguousarray(sign_off, dtype=np.float64).reshape(-1, 4)
     h = _P()
-    try:
+    with Batch.upload(ctx, a) as ba, Batch.upload(ctx, b) as bb:
         check(lib().epid_divide(ctx.handle, ba.handle, bb.handle, _ptr(so), C.byref(h)))
-        out = Batch(ctx, h)
-        try:
+        with Batch(ctx, h) as out:
             r = out.download()
-        finally:
-            out.free()
-    finally:
-        ba.free()
-        bb.free()
     return r[0] if squeeze else r
 
 
 def dlg_analyze(ctx: Context, frames, bottom, top, c0: int, c1: int, planned):
     """-> (measured [n, nleaf], slope [n], intercept [n], dlg [n]) for uint16 frames."""
-    b, own = _as_batch(ctx, frames, (np.dtype(np.uint16),))
-    (n, _, _), _ = b.shape_dtype
     bot = np.ascontiguousarray(bottom, dtype=np.int32)
     tp = np.ascontiguousarray(top, dtype=np.int32)
     pl = np.ascontiguousarray(planned, dtype=np.float64)
     nleaf = len(bot)
-    meas, slope, icpt, dlg = np.empty((n, nleaf)), np.empty(n), np.empty(n), np.empty(n)
-    try:
+    with batch_for(ctx, frames, np.uint16) as b:
+        (n, _, _), _ = b.shape_dtype
+        meas, slope, icpt, dlg = np.empty((n, nleaf)), np.empty(n), np.empty(n), np.empty(n)
         check(lib().epid_dlg_analyze(ctx.handle, b.handle, nleaf, _ptr(bot), _ptr(tp), int(c0), int(c1), _ptr(pl), _ptr(meas), _ptr(slope),
                                      _ptr(icpt), _ptr(dlg)))
-    finally:
-        if own:
-            b.free()
     return meas, slope, icpt, dlg
 
 
 def global_locate(ctx: Context, frames, params: LocateParams, region_cap: int = 1024):
     """Whole-frame threshold sweep: -> list (per frame) of REGION_DTYPE arrays in the reference's visiting order."""
-    b, own = _as_batch(ctx, frames, (np.dtype(np.uint16),))
-    (n, _, _), _ = b.shape_dtype
-    regs = np.zeros((n, region_cap), REGION_DTYPE)
-    counts, flags = np.zeros(n, np.int32), np.zeros(n, np.int32)
-    try:
+    with batch_for(ctx, frames, np.uint16) as b:
+        (n, _, _), _ = b.shape_dtype
+        regs = np.zeros((n, region_cap), REGION_DTYPE)
+        counts, flags = np.zeros(n, np.int32), np.zeros(n, np.int32)
         check(lib().epid_global_locate(ctx.handle, b.handle, C.byref(params), _ptr(regs), int(region_cap), _ptr(counts), _ptr(flags)))
-    finally:
-        if own:
-            b.free()
     if (flags != 0).any():
         raise MemoryError(f"global locator: device lists overflowed (flags {flags.tolist()}); raise region_cap or pre-filter the frame")
     return [regs[i, : counts[i]].copy() for i in range(n)]
@@ -1012,17 +905,11 @@ def canny(ctx: Context, image: np.ndarray, sigma: float = 1.0, low_threshold: fl
     a = np.ascontiguousarray(image, dtype=np.float64)
     squeeze = a.ndim == 2
     w, lw = gaussian_kernel1d(float(sigma))
-    b = Batch.upload(ctx, a)
     h = _P()
-    try:
+    with Batch.upload(ctx, a) as b:
         check(lib().epid_canny(ctx.handle, b.handle, _ptr(w), int(lw), float(low_threshold), float(high_threshold), C.byref(h)))
-        out = Batch(ctx, h)
-        try:
+        with Batch(ctx, h) as out:
             r = out.download()
-        finally:
-            out.free()
-    finally:
-        b.free()
     r = r.astype(bool)
     return r[0] if squeeze else r
 
@@ -1031,12 +918,9 @@ def hough_line(ctx: Context, edges: np.ndarray, theta: np.ndarray):
     """skimage.transform.hough_line: -> (accumulator Batch [1, 2 * offset + 1, ntheta] int32 on the device, offset)"""
     e = np.ascontiguousarray(edges).astype(np.uint8)
     th = np.ascontiguousarray(theta, dtype=np.float64)
-    b = Batch.upload(ctx, e)
     h, off = _P(), C.c_int32()
-    try:
+    with Batch.upload(ctx, e) as b:
         check(lib().epid_hough_line(ctx.handle, b.handle, len(th), _ptr(th), C.byref(h), C.byref(off)))
-    finally:
-        b.free()
     return Batch(ctx, h), off.value
 
 
@@ -1059,14 +943,10 @@ def gather_i32(ctx: Context, img: Batch, yx: np.ndarray) -> np.ndarray:
 
 def weighted_centroid(ctx: Context, frames):
     """(cx, cy, total) arrays of length n: sum(x * a) / sum(a), sum(y * a) / sum(a), sum(a)."""
-    b, own = _as_batch(ctx, frames)
-    (n, _, _), _ = b.shape_dtype
-    cx, cy, tot = np.empty(n), np.empty(n), np.empty(n)
-    try:
+    with batch_for(ctx, frames) as b:
+        (n, _, _), _ = b.shape_dtype
+        cx, cy, tot = np.empty(n), np.empty(n), np.empty(n)
         check(lib().epid_weighted_centroid(ctx.handle, b.handle, _ptr(cx), _ptr(cy), _ptr(tot)))
-    finally:
-        if own:
-            b.free()
     return cx, cy, tot
 
 
@@ -1076,17 +956,14 @@ def circle_profile(ctx: Context, image: np.ndarray, center, radius: float, start
     a = np.ascontiguousarray(image)
     if a.dtype not in (np.uint8, np.uint16, np.float32, np.float64):
         a = a.astype(np.float64)
-    b = Batch.upload(ctx, a)
     rmax = radius * (1 + width_ratio) if collapsed else radius
     cap = int(np.ceil(2 * np.pi * rmax * sampling_ratio)) + 8
     prof, xl, yl = np.empty(cap), np.empty(cap), np.empty(cap)
     cnt = C.c_int32()
-    try:
+    with Batch.upload(ctx, a) as b:
         check(lib().epid_circle_profile(ctx.handle, b.handle, float(center[0]), float(center[1]), float(radius), float(start_angle),
                                         1 if ccw else 0, float(sampling_ratio), 1 if collapsed else 0, float(width_ratio),
                                         int(num_profiles), cap, _ptr(prof), _ptr(xl), _ptr(yl), C.byref(cnt)))
-    finally:
-        b.free()
     c = cnt.value
     return prof[:c].copy(), xl[:c].copy(), yl[:c].copy()
 

@@ -20,7 +20,7 @@ from ..core.image import load
 def _prominent_peaks(ctx, accum, rows: int, cols: int, min_xdistance: int, min_ydistance: int, threshold=None, num_peaks=np.inf):
     """skimage's _prominent_peaks on a device accumulator: -> (values, column indices, row indices)"""
     cand, gmax, filtered = nat.hough_candidates(ctx, accum, min_xdistance, min_ydistance, threshold)
-    try:
+    with filtered:
         if threshold is None:
             threshold = 0.5 * gmax
         # 8-connected components of the candidate cells (sparse), numbered in raster order of their first cell like skimage.label
@@ -53,8 +53,6 @@ def _prominent_peaks(ctx, accum, rows: int, cols: int, min_xdistance: int, min_y
         props = sorted(props, key=lambda p: p[0])[::-1]
         centers = np.array([[int(np.round(p[1])), int(np.round(p[2]))] for p in props], dtype=np.int32).reshape(-1, 2)
         values = nat.gather_i32(ctx, filtered, centers) if len(centers) else np.zeros(0, np.int32)
-    finally:
-        filtered.free()
     peaks, ys, xs = [], [], []
     zeroed: set[tuple[int, int]] = set()      # accumulator cells an accepted peak has zeroed in the reference's img_max
     yext, xext = np.mgrid[-min_ydistance: min_ydistance + 1, -min_xdistance: min_xdistance + 1]
@@ -110,11 +108,9 @@ class JawOrthogonality:
         # classic straight-line Hough transform at a precision of 0.05 degree
         tested_angles = np.linspace(-np.pi / 2, np.pi / 2, num=360 * 10, endpoint=False)
         accum, offset = nat.hough_line(ctx, edge_image, tested_angles)
-        try:
+        with accum:
             d = np.linspace(-offset, offset, 2 * offset + 1)
             _, angles, dists = hough_line_peaks(ctx, accum, tested_angles, d)
-        finally:
-            accum.free()
         if len(angles) < 4:
             raise IndexError(f"only {len(angles)} lines were found; a square field has four")      # the reference fails indexing [2] / [3]
         sorted_idx = np.argsort(np.abs(angles))

@@ -48,19 +48,12 @@ def _run(a, fn, *args):
     a = _coerce(a)
     a3, shape = _as3d(a)
     ctx = _ctx()
-    b = nat.Batch.upload(ctx, a3)
-    try:
-        out = b._unary(fn, *args)
-        try:
-            res = out.download()
-            if res.size == int(np.prod(shape)):
-                return res.reshape(shape)
-            # shape-changing operators (zoom): drop the batch / row axes the input did not have
-            return res.reshape(res.shape[-1]) if len(shape) == 1 else (res[0] if len(shape) == 2 else res)
-        finally:
-            out.free()
-    finally:
-        b.free()
+    with nat.Batch.upload(ctx, a3) as b, b._unary(fn, *args) as out:
+        res = out.download()
+    if res.size == int(np.prod(shape)):
+        return res.reshape(shape)
+    # shape-changing operators (zoom): drop the batch / row axes the input did not have
+    return res.reshape(res.shape[-1]) if len(shape) == 1 else (res[0] if len(shape) == 2 else res)
 
 
 def geometric_center_idx(array: np.ndarray) -> float:  # :38-44
@@ -96,18 +89,12 @@ def ground_with_min(array: np.ndarray, value: float = 0):
     a = _coerce(np.asarray(array))
     a3, shape = _as3d(a)
     ctx = _ctx()
-    b = nat.Batch.upload(ctx, a3)
     mins = np.empty(a3.shape[0], np.float64)
-    try:
-        h = C.c_void_p()
+    h = C.c_void_p()
+    with nat.Batch.upload(ctx, a3) as b:
         nat.check(nat.lib().epid_ground(ctx.handle, b.handle, float(value), C.byref(h), mins.ctypes.data_as(C.c_void_p)))
-        out = nat.Batch(ctx, h)
-        try:
+        with nat.Batch(ctx, h) as out:
             res = out.download().reshape(shape)
-        finally:
-            out.free()
-    finally:
-        b.free()
     mn = a.dtype.type(mins[0]) if a3.shape[0] == 1 else mins.astype(a.dtype)
     return res, mn
 
@@ -240,11 +227,8 @@ def _stats(array: np.ndarray, percentiles=()):
         raise TypeError("exact frame statistics are implemented for uint8/uint16 frames")
     a3, _ = _as3d(_coerce(a))
     ctx = _ctx()
-    b = nat.Batch.upload(ctx, a3)
-    try:
+    with nat.Batch.upload(ctx, a3) as b:
         return nat.frame_stats(ctx, b, percentiles=percentiles)
-    finally:
-        b.free()
 
 
 def percentile(array: np.ndarray, q):

@@ -306,17 +306,9 @@ class BaseImage:
 
         ref, comp = prepared(self), prepared(comparison_image)
         ctx = nat.Context.default()
-        rb = nat.Batch.upload(ctx, ref[None])
-        cb = nat.Batch.upload(ctx, comp[None])
-        try:
-            out = rb._unary2(nat.lib().epid_gamma, cb, float(threshold * np.max(ref)), doseTA / 100.0, float(self.dpmm * distTA))
-            try:
+        with nat.Batch.upload(ctx, ref[None]) as rb, nat.Batch.upload(ctx, comp[None]) as cb:
+            with rb._unary2(nat.lib().epid_gamma, cb, float(threshold * np.max(ref)), doseTA / 100.0, float(self.dpmm * distTA)) as out:
                 return out.download()[0]
-            finally:
-                out.free()
-        finally:
-            rb.free()
-            cb.free()
 
     def compute(self, metrics):
         """core/image.py:1022-1054: inject this image into the metric(s), calculate, store under a unique name."""

@@ -334,28 +334,16 @@ def analyze_batch(frames, dpmm: float, *, device: int | None = None, filter: int
     params = None if per_profile else make_params(dpmm, **kwargs)
     protocol = kwargs.get("protocol", Protocol.VARIAN)
     protocol = Protocol[protocol] if isinstance(protocol, str) else protocol
-    own = None
-    if not isinstance(frames, nat.Batch):
-        a = np.asarray(frames)
-        if a.dtype != np.uint16:
-            raise TypeError("field analysis frames must be uint16")
-        own = frames = nat.Batch.upload(ctx, a)
-    try:
+    with nat.batch_for(ctx, frames, np.uint16) as frames:
         if filter:
-            filtered = frames._unary(nat.lib().epid_median_filter, int(filter))   # image.filter(size=filter) (field_analysis.py:466)
-            try:
+            with frames._unary(nat.lib().epid_median_filter, int(filter)) as filtered:   # image.filter(size=filter) (field_analysis.py:466)
                 if per_profile:
                     return _analyze_per_profile(ctx, filtered, dpmm, kwargs)
                 rows = nat.field_analyze(ctx, filtered, params)
-            finally:
-                filtered.free()
         elif per_profile:
             return _analyze_per_profile(ctx, frames, dpmm, kwargs)
         else:
             rows = nat.field_analyze(ctx, frames, params)
-    finally:
-        if own is not None:
-            own.free()
     return FieldBatchResult(rows, protocol)
 
 

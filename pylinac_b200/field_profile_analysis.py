@@ -88,13 +88,9 @@ class FieldProfileAnalysis(ResultsDataMixin[FieldProfileResult]):
         self._centering = convert_to_enum(centering, Centering)
         metrics = default_metrics() if metrics is None else metrics
         ctx = nat.Context.default()
-        shared = getattr(self, "_shared", None)
-        batch = shared[0].batch if shared else nat.Batch.upload(ctx, self._frame_u16()[None])
-        try:
+        frames = self._shared[0].batch if hasattr(self, "_shared") else self._frame_u16()
+        with nat.batch_for(ctx, frames) as batch:
             x_values, y_values = self._get_profile_values(ctx, batch, position, x_width, y_width)
-        finally:
-            if not shared:
-                batch.free()
         cls = PROFILES[self._edge_type]
         self.x_profile = cls(values=x_values, dpmm=self.image.dpmm, normalization=normalization, ground=ground, **kwargs)
         self.x_profile.compute(metrics=metrics)
@@ -196,24 +192,21 @@ def analyze_batch(frames, dpmm: float, *, device: int | None = None, sid: float 
     if a.dtype != np.uint16:
         raise TypeError("field-profile frames must be uint16")
     ctx = nat.Context.default(device)
-    batch = nat.Batch.upload(ctx, a)
     out = []
-    try:
-        shared = _BatchStats(ctx, batch)
+    with nat.Batch.upload(ctx, a) as batch:
+        stats = _BatchStats(ctx, batch)
         for i in range(len(a)):
             f = FieldProfileAnalysis.__new__(FieldProfileAnalysis)
             f.image = image.ArrayImage(a[i], dpi=dpmm * 25.4 * 1000.0 / sid, sid=sid)
             f._is_analyzed = False
             f._warnings = []
-            f._flipped = shared.hist_inverted(i)  # check_inversion_by_histogram() of the constructor
+            f._flipped = stats.hist_inverted(i)  # check_inversion_by_histogram() of the constructor
             if f._flipped:
                 f.image.invert()
-            f._shared = (shared, i)
+            f._shared = (stats, i)
             f.analyze(**analyze_kwargs)
             del f._shared
             out.append(f)
-    finally:
-        batch.free()
     return out
 
 

@@ -342,29 +342,16 @@ def _gamma_maps(actual: nat.Batch, expected: nat.Batch, doseTA, distTA, threshol
     lib = nat.lib()
 
     def prepared(b: nat.Batch) -> nat.Batch:
-        inv, _ = nat.hist_invert(ctx, b)
-        try:
-            h = nat._P()
+        h = nat._P()
+        with nat.hist_invert(ctx, b)[0] as inv:
             nat.check(lib.epid_ground(ctx.handle, inv.handle, 0.0, nat.C.byref(h), None))
-            grounded = nat.Batch(ctx, h)
-        finally:
-            inv.free()
-        try:
+        with nat.Batch(ctx, h) as grounded:
             return grounded._unary(lib.epid_normalize, 1, 0.0)
-        finally:
-            grounded.free()
 
-    ref = prepared(actual)
-    try:
-        comp = prepared(expected)
-        try:
-            # after normalize() the reference's max is exactly 1.0 (or nan for a constant map, where every pixel is nan already)
-            dpmm = (25.4 / resolution) / 25.4
-            g = ref._unary2(lib.epid_gamma, comp, float(threshold * 1.0), doseTA / 100.0, float(dpmm * distTA))
-        finally:
-            comp.free()
-    finally:
-        ref.free()
+    with prepared(actual) as ref, prepared(expected) as comp:
+        # after normalize() the reference's max is exactly 1.0 (or nan for a constant map, where every pixel is nan already)
+        dpmm = (25.4 / resolution) / 25.4
+        g = ref._unary2(lib.epid_gamma, comp, float(threshold * 1.0), doseTA / 100.0, float(dpmm * distTA))
     s, cnt, passing = nat.gamma_stats(ctx, g)
     avg, pct = [], []
     with np.errstate(invalid="ignore", divide="ignore"):

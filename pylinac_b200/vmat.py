@@ -449,11 +449,8 @@ class DRCS(VMATBase):
         for img in (image1, image2):
             tmp = image.ArrayImage(np.ascontiguousarray(frame_u16(img, "VMAT")))
             tmp.filter(size=10, kind="median")
-            b = nat.Batch.upload(ctx, tmp.array)
-            try:
+            with nat.Batch.upload(ctx, tmp.array) as b:
                 st = nat.frame_stats(ctx, b)       # exact integer sum and max of the filtered frame
-            finally:
-                b.free()
             sums.append(float(st["sum"][0]) / float(st["max"][0]))       # normalize(...).sum()
         if sums[0] > sums[1]:
             self.open_image, self.dmlc_image = image1, image2

@@ -329,29 +329,14 @@ def cbct_frames(volume, ratio: float, *, device: int | None = None):
     (epid_cbct_views).  Returns [(uint16 device Batch, set indices)] in the order of the reference's file names G=0, G=180, G=270,
     G=90 (top, bottom, left, right): one batch of 4 for square slices, else one per frame shape."""
     ctx = nat.Context.default(device)
-    vol = nat.Batch.upload(ctx, volume)
-    try:
+    with nat.Batch.upload(ctx, volume) as vol:
         colmax, rowmax = nat.stack_mip(ctx, vol)
-    finally:
-        vol.free()
-    try:
-        zc = colmax._unary(nat.lib().epid_zoom, float(ratio), 1, 3)     # order 1, mode 'nearest' | grid_mode
-        try:
-            zr = rowmax._unary(nat.lib().epid_zoom, float(ratio), 1, 3)
-        except BaseException:
-            zc.free()
-            raise
-    finally:
-        colmax.free()
-        rowmax.free()
-    try:
-        src = np.asarray(volume).dtype
+    src = np.asarray(volume).dtype
+    zoom = nat.lib().epid_zoom        # arguments (ratio, 1, 3): order 1, mode 'nearest' | grid_mode
+    with colmax, rowmax, colmax._unary(zoom, float(ratio), 1, 3) as zc, rowmax._unary(zoom, float(ratio), 1, 3) as zr:
         if zc.shape_dtype[0] == zr.shape_dtype[0]:
             return [(nat.cbct_views(ctx, zr, zc, src), [0, 1, 2, 3])]
         return [(nat.cbct_views(ctx, zr, None, src), [0, 1]), (nat.cbct_views(ctx, zc, None, src), [2, 3])]
-    finally:
-        zc.free()
-        zr.free()
 
 
 # ---------------------------------------------------------------------------------------------------------------- set level

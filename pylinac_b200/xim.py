@@ -245,9 +245,7 @@ def decode_file(hd: XimHeader, device: int | None = None) -> np.ndarray:
     arena = nat.pinned_empty((total,), np.uint8)
     _fill(arena, hd, int(desc[0, 0]), int(desc[0, 2]))
     batch, status = decode_arena(arena, desc, h, w, bpp, None, device)
-    try:
+    with batch:
         raise_status(int(status[0]), hd.path)
         a = batch.download()[0]
-    finally:
-        batch.free()
     return a.astype(np.int8) if bpp == 1 else a
