@@ -506,6 +506,18 @@ int32_t epid_rotate(epid_ctx* ctx, const epid_batch* in, double angle_deg, int32
  * one fused kernel; out: a new float64 batch (nan where the reference is below the threshold). */
 int32_t epid_gamma(epid_ctx* ctx, const epid_batch* ref, const epid_batch* comp, double threshold_abs, double dose_frac, double dist_px,
                    epid_batch** out);
+/* pylinac.core.gamma.gamma_2d (core/gamma.py:229-330), Low et al. 2004 Table I, for n (reference, evaluation) pairs: dose_frac =
+ * dose_to_agreement / 100 times reference.max() (global_dose != 0, taken on the device per pair; a nan makes it nan) or times the
+ * reference elementwise; threshold = dose_threshold / 100, compared with the normalised reference; pixels at or above it take the
+ * minimum over the disk of dist2[k] + (eval_n - ref_n)^2 with the evaluation clamped to its own shape (np.pad mode 'edge'), capped
+ * at cap (cap2 = cap**2 as the caller computes it); others take fill_value.  offsets: [n_off][2] (row, col) of skimage.draw.disk((0,
+ * 0), dta + 1) and dist2 their (r / dta)**2 + (c / dta)**2, sorted by dist2, raster order breaking ties.  Any dtype; numpy 2
+ * promotion (a float32 reference normalises in float32).  Global mode needs an evaluation at least the reference's shape, local mode
+ * equal shapes.  full_search != 0 disables the exact early exit.  out: a new float64 batch of the reference's shape, bit-identical to
+ * the reference. */
+int32_t epid_gamma2d(epid_ctx* ctx, const epid_batch* ref, const epid_batch* eval, double dose_frac, double threshold, double cap,
+                     double cap2, double fill_value, int32_t global_dose, const int32_t* offsets, const double* dist2, int32_t n_off,
+                     int32_t full_search, epid_batch** out);
 
 /* ----------------------------------------------------------------------------------------- ROI statistics / weighted centroid
  * RectangleROI.mean / std / min / max (core/roi.py:533-706): pixels of a rectangle given by its corners verts_xy[nroi][4][(x, y)]

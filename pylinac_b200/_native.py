@@ -288,6 +288,8 @@ _SIGNATURES = {
     "epid_zoom": [_P, _P, C.c_double, C.c_int32, C.c_int32, C.POINTER(_P)],
     "epid_rotate": [_P, _P, C.c_double, C.c_int32, C.POINTER(_P)],
     "epid_gamma": [_P, _P, _P, C.c_double, C.c_double, C.c_double, C.POINTER(_P)],
+    "epid_gamma2d": [_P, _P, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int32, _P, _P, C.c_int32, C.c_int32,
+                     C.POINTER(_P)],
     "epid_disk_locate": [_P, _P, _P, _P],
     "epid_roi_stats": [_P, _P, C.c_int32, _P, _P, _P, _P, _P, _P],
     "epid_weighted_centroid": [_P, _P, _P, _P, _P],
@@ -619,6 +621,17 @@ def gamma_stats(ctx: Context, gamma: Batch) -> tuple[np.ndarray, np.ndarray, np.
     s, c, p = np.zeros(n), np.zeros(n, np.int64), np.zeros(n, np.int64)
     check(lib().epid_gamma_stats(ctx.handle, gamma.handle, _ptr(s), _ptr(c), _ptr(p)))
     return s, c, p
+
+
+def gamma2d(ctx: Context, ref: Batch, ev: Batch, dose_frac: float, threshold: float, cap: float, cap2: float, fill_value: float,
+            global_dose: bool, offsets: np.ndarray, dist2: np.ndarray, full_search: bool = False) -> Batch:
+    """epid_gamma2d -> float64 gamma maps [n, h, w] (device batch); offsets int32 [k, 2] and dist2 float64 [k] sorted by dist2"""
+    o = np.ascontiguousarray(offsets, dtype=np.int32)
+    d = np.ascontiguousarray(dist2, dtype=np.float64)
+    h = _P()
+    check(lib().epid_gamma2d(ctx.handle, ref.handle, ev.handle, float(dose_frac), float(threshold), float(cap), float(cap2),
+                             float(fill_value), int(bool(global_dose)), _ptr(o), _ptr(d), len(d), int(bool(full_search)), C.byref(h)))
+    return Batch(ctx, h)
 
 
 def _unsupported_as_not_implemented(rc):
