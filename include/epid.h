@@ -518,6 +518,24 @@ int32_t epid_gamma(epid_ctx* ctx, const epid_batch* ref, const epid_batch* comp,
 int32_t epid_gamma2d(epid_ctx* ctx, const epid_batch* ref, const epid_batch* eval, double dose_frac, double threshold, double cap,
                      double cap2, double fill_value, int32_t global_dose, const int32_t* offsets, const double* dist2, int32_t n_off,
                      int32_t full_search, epid_batch** out);
+/* pylinac.core.gamma.gamma_geometric (core/gamma.py:105-226, Ju et al. 2008) for n profile pairs, all arrays in host memory.  Pair i
+ * has the normalised evaluation samples eval_x / eval_y[eval_off[i] .. eval_off[i + 1]] (strictly monotonic x, decreasing[i] != 0 when
+ * decreasing, at least 2 samples when the pair has points) and the normalised evaluated reference points ref_x / ref_y[pt_off[i] ..
+ * pt_off[i + 1]].  dta is the distance to agreement the reference subtracts from the normalised x, cap the gamma cap.  gamma[k]: the
+ * capped minimum segment distance of point k, bit-identical to the reference; svd_fail[i] != 0 where a segment of pair i has a nan
+ * V^T V (the reference's pinv raises LinAlgError).  One upload, one kernel, one download. */
+int32_t epid_gamma_geometric(epid_ctx* ctx, int32_t n, const int64_t* eval_off, const int64_t* pt_off, const int32_t* decreasing,
+                             const double* eval_x, const double* eval_y, const double* ref_x, const double* ref_y, double dta, double cap,
+                             double* gamma, int32_t* svd_fail);
+/* pylinac.core.gamma.gamma_1d (core/gamma.py:333-460, Low et al. 2004) for n profile pairs, all arrays in host memory: eval_x / eval_y
+ * are each pair's evaluation coordinates and values sorted by x (interp1d's stable sort; at least 2 when the pair has points), ref_x /
+ * ref_y the evaluated reference points, dose_ta2[k] the dose criterion squared of point k (float32 values where dose_f32[i] != 0: the
+ * dose term then divides in float32).  Each point samples np.linspace(ref_x - dta, ref_x + dta, num), interpolates the evaluation
+ * there (interp1d linear, extrapolating) and takes min sqrt(dist**2 / dta2 + dose**2 / dose_ta2), capped at cap.  Outputs gamma[k],
+ * samples[k * num + j] and sample_x[k * num + j].  One upload, one kernel, one download. */
+int32_t epid_gamma1d(epid_ctx* ctx, int32_t n, const int64_t* eval_off, const int64_t* pt_off, const int32_t* dose_f32, const double* eval_x,
+                     const double* eval_y, const double* ref_x, const double* ref_y, const double* dose_ta2, double dta, double dta2,
+                     int32_t num, double cap, double* gamma, double* samples, double* sample_x);
 
 /* ----------------------------------------------------------------------------------------- ROI statistics / weighted centroid
  * RectangleROI.mean / std / min / max (core/roi.py:533-706): pixels of a rectangle given by its corners verts_xy[nroi][4][(x, y)]

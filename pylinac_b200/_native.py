@@ -290,6 +290,8 @@ _SIGNATURES = {
     "epid_gamma": [_P, _P, _P, C.c_double, C.c_double, C.c_double, C.POINTER(_P)],
     "epid_gamma2d": [_P, _P, _P, C.c_double, C.c_double, C.c_double, C.c_double, C.c_double, C.c_int32, _P, _P, C.c_int32, C.c_int32,
                      C.POINTER(_P)],
+    "epid_gamma_geometric": [_P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, C.c_double, C.c_double, _P, _P],
+    "epid_gamma1d": [_P, C.c_int32, _P, _P, _P, _P, _P, _P, _P, _P, C.c_double, C.c_double, C.c_int32, C.c_double, _P, _P, _P],
     "epid_disk_locate": [_P, _P, _P, _P],
     "epid_roi_stats": [_P, _P, C.c_int32, _P, _P, _P, _P, _P, _P],
     "epid_weighted_centroid": [_P, _P, _P, _P, _P],
@@ -632,6 +634,38 @@ def gamma2d(ctx: Context, ref: Batch, ev: Batch, dose_frac: float, threshold: fl
     check(lib().epid_gamma2d(ctx.handle, ref.handle, ev.handle, float(dose_frac), float(threshold), float(cap), float(cap2),
                              float(fill_value), int(bool(global_dose)), _ptr(o), _ptr(d), len(d), int(bool(full_search)), C.byref(h)))
     return Batch(ctx, h)
+
+
+def _f64(a):
+    return np.ascontiguousarray(a, dtype=np.float64)
+
+
+def _i64(a):
+    return np.ascontiguousarray(a, dtype=np.int64)
+
+
+def gamma_geometric(ctx: Context, eval_off, pt_off, decreasing, eval_x, eval_y, ref_x, ref_y, dta: float,
+                    cap: float) -> tuple[np.ndarray, np.ndarray]:
+    """epid_gamma_geometric -> (gamma float64 [points], svd_fail int32 [pairs]); packed host arrays, CSR offsets per pair"""
+    eo, po, dec = _i64(eval_off), _i64(pt_off), np.ascontiguousarray(decreasing, dtype=np.int32)
+    ex, ey, rx, ry = _f64(eval_x), _f64(eval_y), _f64(ref_x), _f64(ref_y)
+    n = len(eo) - 1
+    g, fail = np.empty(int(po[-1])), np.zeros(n, np.int32)
+    check(lib().epid_gamma_geometric(ctx.handle, n, _ptr(eo), _ptr(po), _ptr(dec), _ptr(ex), _ptr(ey), _ptr(rx), _ptr(ry), float(dta),
+                                     float(cap), _ptr(g), _ptr(fail)))
+    return g, fail
+
+
+def gamma1d(ctx: Context, eval_off, pt_off, dose_f32, eval_x, eval_y, ref_x, ref_y, dose_ta2, dta: float, dta2: float, num: int,
+            cap: float) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+    """epid_gamma1d -> (gamma [points], samples [points, num], sample x [points, num]), float64; packed host arrays, CSR offsets"""
+    eo, po, f32 = _i64(eval_off), _i64(pt_off), np.ascontiguousarray(dose_f32, dtype=np.int32)
+    ex, ey, rx, ry, d2 = _f64(eval_x), _f64(eval_y), _f64(ref_x), _f64(ref_y), _f64(dose_ta2)
+    n, k = len(eo) - 1, int(po[-1])
+    g, s, x = np.empty(k), np.empty((k, num)), np.empty((k, num))
+    check(lib().epid_gamma1d(ctx.handle, n, _ptr(eo), _ptr(po), _ptr(f32), _ptr(ex), _ptr(ey), _ptr(rx), _ptr(ry), _ptr(d2), float(dta),
+                             float(dta2), int(num), float(cap), _ptr(g), _ptr(s), _ptr(x)))
+    return g, s, x
 
 
 def _unsupported_as_not_implemented(rc):

@@ -244,6 +244,20 @@ class SingleProfile(ProfileMixin):
         self.x_indices = self._x_explicit if self._x_explicit is not None else \
             np.linspace(float(r["x_start"]), float(r["x_stop"]), num=int(r["n"]))
 
+    def gamma(self, evaluation_profile, distance_to_agreement: int = 1, dose_to_agreement: float = 1, gamma_cap_value: float = 2,
+              dose_threshold: float = 5, global_dose: bool = True, fill_value: float = np.nan) -> np.ndarray:
+        """core/profile.py:1939-1993: ``core.gamma.gamma_1d`` of the two profiles over their ``x_indices`` (note the argument order:
+        distance first); both profiles need ``dpmm``."""
+        from .gamma import gamma_1d
+
+        if not self.dpmm or not evaluation_profile.dpmm:
+            raise ValueError("At least one profile does not have the dpmm attribute. Physical spacing cannot be determined. Set it "
+                             "before performing gamma analysis.")
+        return gamma_1d(reference=self.values, evaluation=evaluation_profile.values, reference_coordinates=self.x_indices,
+                        evaluation_coordinates=evaluation_profile.x_indices, dose_to_agreement=dose_to_agreement,
+                        distance_to_agreement=distance_to_agreement, gamma_cap_value=gamma_cap_value, global_dose=global_dose,
+                        dose_threshold=dose_threshold, fill_value=fill_value)[0]
+
     # -- _interpolate (core/profile.py:1306-1360) for the cases the device interpolation does not cover
     def _presample(self, raw: np.ndarray, x_values):
         x = np.arange(len(raw), dtype=np.float64) if x_values is None else np.asarray(x_values, dtype=np.float64)
@@ -802,6 +816,26 @@ class PhysicalProfileMixin:
     def as_simple_profile(self):
         """core/profile.py:932-949: the non-physical parent class over the physical x positions"""
         return type(self).__bases__[-1](values=self.values, x_values=self.physical_x_values)
+
+    def gamma(self, evaluation_profile, dose_to_agreement: float = 3, distance_to_agreement: float = 3, gamma_cap_value: float = 2,
+              dose_threshold: float = 5, fill_value: float = np.nan, return_profiles: bool = False):
+        """core/profile.py:822-874: ``core.gamma.gamma_geometric`` of copies of both profiles, each shifted so that its geometric
+        centre is at x = 0, over their physical x values.  ``return_profiles=True`` returns ``(gamma, reference, evaluation)`` with
+        those copies."""
+        import copy
+
+        from .gamma import gamma_geometric
+
+        if not isinstance(evaluation_profile, PhysicalProfileMixin):
+            raise ValueError("The evaluation profile must also be a physical profile.")
+        reference, evaluation = copy.deepcopy(self), copy.deepcopy(evaluation_profile)
+        reference.x_values = reference.x_values - reference.geometric_center_idx
+        evaluation.x_values = evaluation.x_values - evaluation.geometric_center_idx
+        gamma = gamma_geometric(reference=reference.values, reference_coordinates=reference.physical_x_values,
+                                evaluation=evaluation.values, evaluation_coordinates=evaluation.physical_x_values,
+                                dose_to_agreement=dose_to_agreement, distance_to_agreement=distance_to_agreement,
+                                gamma_cap_value=gamma_cap_value, dose_threshold=dose_threshold, fill_value=fill_value)
+        return (gamma, reference, evaluation) if return_profiles else gamma
 
     def as_resampled(self, interpolation_resolution_mm: float = 0.1, order: int = 3, grid: bool = True):
         """core/profile.py:951-1013: resample to ``interpolation_resolution_mm`` per sample.  ``grid`` treats samples as pixels of
