@@ -759,6 +759,42 @@ int32_t epid_lightrad_analyze(epid_ctx* ctx, const epid_batch* frames, const epi
 int32_t epid_lightrad_stages(epid_ctx* ctx, const epid_batch* frames, const epid_lr_params* p, epid_lr_result* results,
                              uint16_t* filtered, uint16_t* equalised, uint16_t* equalised_filtered, int64_t* info);
 
+/* ----------------------------------------------------------------------------------------- nuclear medicine
+ * pylinac.nuclear.PlanarUniformity (nuclear.py:151-500): NEMA integral and differential uniformity of uint16 gamma-camera flood frames,
+ * bit-identical to the reference.  Per frame: bin x bin block sums (zero-padded bottom / right), the 9-point filter as the integer
+ * S = 16 x filtered value with the outer rows / columns zeroed, the threshold (mean of the values above 10 % of the max, times
+ * `threshold`), the stray-pixel stencil, the largest 4-connected component (lowest label on ties) and its longest bounding-box side L,
+ * erosion k = rint(erode[k] * L) with erode = 1 - size computed by the caller, FOV k = exact EDT > erosion / 2, and the uniformities of
+ * the non-zero FOV pixels.  Index 0 of every pair is the UFOV, 1 the CFOV; du_* are indexed [2 * fov + axis], axis 0 being windows of
+ * `window` pixels down a column.  The row is a plain struct (not a typedef): its layout is checked by tests/test_nuclear_host.py. */
+enum { EPID_NM_OK = 0, EPID_NM_NO_COMPONENT = 1 /* no foreground pixel survives the cleaning (get_fov raises) */ };
+struct epid_nm_result { /* one per frame */
+    int32_t status;
+    int32_t longest;                   /* L */
+    int32_t erosion[2];
+    int32_t n_fov[2];                  /* non-zero FOV pixels (0: integral_uniformity raises) */
+    int32_t max_index[2];              /* first raster index (row * wb + col) of the FOV maximum / minimum */
+    int32_t min_index[2];
+    int32_t du_count[4];               /* windows holding a FOV pixel (0: differential_uniformity raises) */
+    int32_t du_index[4];               /* first (i, j) in row-major order of du_max, as i * wb + j */
+    double threshold;                  /* the absolute threshold on S / 16 (nan for a blank frame) */
+    double iu[2];                      /* integral uniformity, % */
+    double du_max[4];                  /* maximum window uniformity, % */
+};
+
+/* frames: uint16 batch; bin: a power of two up to 64; window >= 1.  results: host rows [n].  cleaned (may be NULL): a new float64
+ * batch [n][hb][wb] of S / 16 (the reference's binned_frame); masks (may be NULL): a new uint8 batch [2n][hb][wb], the UFOV and CFOV
+ * masks of frame k at 2k and 2k + 1.  Non-uint16 frames or bins return EPID_ERR_UNSUPPORTED. */
+int32_t epid_nm_uniformity(epid_ctx* ctx, const epid_batch* frames, int32_t bin, double ufov_erode, double cfov_erode, int32_t window,
+                           double threshold, struct epid_nm_result* results, epid_batch** cleaned, epid_batch** masks);
+/* Diagnostic read-back: the launch sequence of epid_nm_uniformity and host planes [n][hb][wb] of S after the filter (filtered), S after
+ * the threshold and stencil (cleaned) and the squared EDT (edt2, -1 for a frame without a component), plus masks [n][2][hb][wb]. */
+int32_t epid_nm_stages(epid_ctx* ctx, const epid_batch* frames, int32_t bin, double ufov_erode, double cfov_erode, int32_t window,
+                       double threshold, struct epid_nm_result* results, uint32_t* filtered, uint32_t* cleaned, int32_t* edt2, uint8_t* masks);
+/* pylinac.nuclear.get_fov on n binary frames (uint8, non-zero = foreground): status, longest, erosion[0] = rint(erode * L) and n_fov[0]
+ * of each row, and mask: a new uint8 batch [2n][h][w] whose frame 2k is the eroded binary of frame k. */
+int32_t epid_nm_fov(epid_ctx* ctx, const epid_batch* binary, double erode, struct epid_nm_result* results, epid_batch** mask);
+
 /* ----------------------------------------------------------------------------------------- multi-GPU (NCCL)
  * The batch shards by frame index with no data-path collective; the only exchange is the final gather of the
  * fixed-size per-frame result structs (SURVEY.md 8e).  id: 128-byte ncclUniqueId created by rank 0. */

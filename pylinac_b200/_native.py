@@ -231,6 +231,14 @@ class LocateParams(C.Structure):
                 ("field_tolerance_mm", C.c_double), ("bb_size_mm", C.c_double), ("rad_size_mm", C.c_double)]
 
 
+NM_OK, NM_NO_COMPONENT = 0, 1
+
+NM_RESULT_DTYPE = np.dtype([
+    ("status", "<i4"), ("longest", "<i4"), ("erosion", "<i4", (2,)), ("n_fov", "<i4", (2,)), ("max_index", "<i4", (2,)),
+    ("min_index", "<i4", (2,)), ("du_count", "<i4", (4,)), ("du_index", "<i4", (4,)), ("threshold", "<f8"), ("iu", "<f8", (2,)),
+    ("du_max", "<f8", (4,))], align=True)
+
+
 REGION_DTYPE = np.dtype([("threshold_index", "<i4"), ("label_root", "<i4"), ("bbox", "<i4", (4,)), ("area", "<f8"), ("area_filled", "<f8"),
                          ("perimeter", "<f8"), ("equivalent_diameter", "<f8"), ("centroid_y", "<f8"), ("centroid_x", "<f8"),
                          ("wcentroid_y", "<f8"), ("wcentroid_x", "<f8")], align=True)
@@ -301,6 +309,9 @@ _SIGNATURES = {
     "epid_global_locate": [_P, _P, C.POINTER(LocateParams), _P, C.c_int32, _P, _P],
     "epid_lightrad_analyze": [_P, _P, C.POINTER(LrParams), _P],
     "epid_lightrad_stages": [_P, _P, C.POINTER(LrParams), _P, _P, _P, _P, _P],
+    "epid_nm_uniformity": [_P, _P, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_double, _P, C.POINTER(_P), C.POINTER(_P)],
+    "epid_nm_stages": [_P, _P, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_double, _P, _P, _P, _P, _P],
+    "epid_nm_fov": [_P, _P, C.c_double, _P, C.POINTER(_P)],
     "epid_canny": [_P, _P, _P, C.c_int32, C.c_double, C.c_double, C.POINTER(_P)],
     "epid_hough_line": [_P, _P, C.c_int32, _P, C.POINTER(_P), C.POINTER(C.c_int32)],
     "epid_hough_candidates": [_P, _P, C.c_int32, C.c_int32, C.c_double, C.c_int32, _P, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
@@ -904,6 +915,51 @@ def lightrad_stages(ctx: Context, frames, params: LrParams) -> dict:
         check(lib().epid_lightrad_stages(ctx.handle, b.handle, C.byref(params), _ptr(res), *[_ptr(a) for a in planes], _ptr(info)))
     return {"results": res, "filtered": planes[0], "equalised": planes[1], "equalised_filtered": planes[2],
             "info": {name: info[:, k] for k, name in enumerate(LR_INFO_FIELDS)}}
+
+
+def nm_uniformity(ctx: Context, frames, bin_size: int, ufov_erode: float, cfov_erode: float, window: int, threshold: float,
+                  arrays: bool = True):
+    """epid_nm_uniformity on uint16 frames (Batch or ndarray [n,h,w] / [h,w]) -> (NM_RESULT_DTYPE rows, cleaned, masks): cleaned is a
+    float64 device Batch [n, hb, wb] and masks a uint8 device Batch [2n, hb, wb] (UFOV, CFOV of each frame), both None when not
+    `arrays`.  Unsupported dtypes and bin sizes raise NotImplementedError."""
+    with batch_for(ctx, frames) as b:
+        (n, _, _), _ = b.shape_dtype
+        res = np.zeros(n, NM_RESULT_DTYPE)
+        hc, hm = _P(), _P()
+        _unsupported_as_not_implemented(lib().epid_nm_uniformity(
+            ctx.handle, b.handle, int(bin_size), float(ufov_erode), float(cfov_erode), int(window), float(threshold), _ptr(res),
+            C.byref(hc) if arrays else None, C.byref(hm) if arrays else None))
+    if not arrays:
+        return res, None, None
+    return res, Batch(ctx, hc), Batch(ctx, hm)
+
+
+def nm_stages(ctx: Context, frames, bin_size: int, ufov_erode: float, cfov_erode: float, window: int, threshold: float) -> dict:
+    """Diagnostic read-back of epid_nm_stages: {"results", "filtered" (uint32 S after the filter), "cleaned" (uint32 S after the
+    threshold and the stray-pixel stencil), "edt2" (int32 squared EDT, -1 for a frame without a component), "masks" (uint8
+    [n, 2, hb, wb])}."""
+    with batch_for(ctx, frames) as b:
+        (n, h, w), _ = b.shape_dtype
+        hb, wb = -(-h // int(bin_size)), -(-w // int(bin_size))
+        res = np.zeros(n, NM_RESULT_DTYPE)
+        filt, clean = np.empty((n, hb, wb), np.uint32), np.empty((n, hb, wb), np.uint32)
+        edt2, masks = np.empty((n, hb, wb), np.int32), np.empty((n, 2, hb, wb), np.uint8)
+        _unsupported_as_not_implemented(lib().epid_nm_stages(
+            ctx.handle, b.handle, int(bin_size), float(ufov_erode), float(cfov_erode), int(window), float(threshold), _ptr(res),
+            _ptr(filt), _ptr(clean), _ptr(edt2), _ptr(masks)))
+    return {"results": res, "filtered": filt, "cleaned": clean, "edt2": edt2, "masks": masks}
+
+
+def nm_fov(ctx: Context, binary: np.ndarray, erode: float) -> tuple[np.ndarray, np.ndarray]:
+    """epid_nm_fov on one 2-D binary frame -> (NM_RESULT_DTYPE row, eroded uint8 mask)"""
+    a = np.ascontiguousarray(binary, dtype=np.uint8)[None]
+    res = np.zeros(1, NM_RESULT_DTYPE)
+    with Batch.upload(ctx, a) as b:
+        h = _P()
+        check(lib().epid_nm_fov(ctx.handle, b.handle, float(erode), _ptr(res), C.byref(h)))
+        with Batch(ctx, h) as m:
+            mask = m.download()[0]
+    return res[0], mask
 
 
 def divide(ctx: Context, num, den, sign_off=None) -> np.ndarray:

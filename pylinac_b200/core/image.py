@@ -735,6 +735,37 @@ class DicomImageStack:
         return len(self.images)
 
 
+class NMImageStack:
+    """core/image.py:2216-2249: the N frames of one nuclear medicine file, each a DicomImage holding the stored frame as is.
+    Every frame is read by one ``dicom.read_nm_frames`` pass into page-locked memory (pageable without a CUDA device)."""
+
+    def __init__(self, path):
+        self.path = path
+        self.metadata = dicom.read_header(path)
+        if self.metadata.get("Modality") != "NM":
+            raise TypeError("The file is not a NM image")
+        shape = (int(self.metadata.get("NumberOfFrames", 1) or 1), int(self.metadata["Rows"]), int(self.metadata["Columns"]))
+        try:
+            out = nat.pinned_empty(shape, self.metadata["PixelDtype"])
+        except nat.NativeError:      # no CUDA device: pageable host memory (only the H2D copy is slower)
+            out = None
+        self._pixels, _ = dicom.read_nm_frames([path], out=out)
+        self.frames = []
+        for pixels in self._pixels:
+            ds = dicom.Dataset(self.metadata)
+            ds.pixel_array = pixels
+            img = DicomImage(ds)
+            img.array = pixels           # the reference assigns the stored frame, without the rescale DicomImage applies
+            self.frames.append(img)
+
+    def as_3d_array(self) -> np.ndarray:
+        """the frames stacked into one [n, h, w] array (a copy)"""
+        return np.stack([i.array for i in self.frames], axis=0)
+
+    def __len__(self):
+        return len(self.frames)
+
+
 class XIM(BaseImage):
     """core/image.py:1105-1318: a Varian .xim image (TrueBeam / Halcyon EPID and kV, IsoCal and MPC exports).  The header and
     property walk is the reference's (pylinac_b200.xim); the compressed pixels are decoded on the GPU (csrc/xim.cu) through the

@@ -323,16 +323,46 @@ def read_frames(paths, out=None, threads: int = 8, headers=None):
         if out.shape != (len(paths),) + shape or out.dtype != dt or not out.flags.c_contiguous:
             raise ValueError(f"out must be a C-contiguous {(len(paths),) + shape} array of {dt}")
 
-        def fill(i):
-            with open(paths[i], "rb", buffering=0) as f:
-                f.seek(headers[i]["PixelOffset"])
-                mv = memoryview(out[i]).cast("B")
-                got = 0
-                while got < len(mv):
-                    k = f.readinto(mv[got:])
-                    if not k:
-                        raise InvalidDicomError(f"{paths[i]}: pixel data is truncated")
-                    got += k
+        list(pool.map(lambda i: _read_pixels(paths[i], headers[i], out[i]), range(len(paths))))
+    return out, headers
 
-        list(pool.map(fill, range(len(paths))))
+
+def _read_pixels(path, header, dst: np.ndarray) -> None:
+    """``readinto`` the pixel bytes of `path` (located by its `header`) straight into the C-contiguous `dst`"""
+    with open(path, "rb", buffering=0) as f:
+        f.seek(header["PixelOffset"])
+        mv = memoryview(dst).cast("B")
+        got = 0
+        while got < len(mv):
+            k = f.readinto(mv[got:])
+            if not k:
+                raise InvalidDicomError(f"{path}: pixel data is truncated")
+            got += k
+
+
+def read_nm_frames(paths, out=None, threads: int = 8):
+    """Batched ingest of multi-frame files (nuclear medicine stacks): every frame of every file, in file then frame order, read with
+    ``readinto`` straight into one [n, rows, cols] array, where n is the files' total NumberOfFrames.  Pass a page-locked array
+    (``_native.pinned_empty``) as `out` for a direct H2D copy.  All files must share rows / columns / stored dtype.  Returns
+    (frames, headers)."""
+    from concurrent.futures import ThreadPoolExecutor
+
+    paths = [str(p) for p in paths]
+    if not paths:
+        raise ValueError("no files")
+    with ThreadPoolExecutor(max(1, min(threads, len(paths)))) as pool:
+        headers = list(pool.map(read_header, paths))
+        h0 = headers[0]
+        shape = (int(h0["Rows"]), int(h0["Columns"]))
+        dt = h0["PixelDtype"]
+        for pth, h in zip(paths, headers):
+            if (int(h["Rows"]), int(h["Columns"])) != shape or h["PixelDtype"] != dt:
+                raise ValueError(f"{pth}: {h['Rows']} x {h['Columns']} {h['PixelDtype']} differs from the first file's {shape} {dt}")
+        counts = [int(h.get("NumberOfFrames", 1) or 1) for h in headers]
+        starts = np.concatenate([[0], np.cumsum(counts)])
+        if out is None:
+            out = np.empty((int(starts[-1]),) + shape, dt)
+        if out.shape != (int(starts[-1]),) + shape or out.dtype != dt or not out.flags.c_contiguous:
+            raise ValueError(f"out must be a C-contiguous {(int(starts[-1]),) + shape} array of {dt}")
+        list(pool.map(lambda i: _read_pixels(paths[i], headers[i], out[starts[i]:starts[i + 1]]), range(len(paths))))
     return out, headers
