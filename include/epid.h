@@ -795,6 +795,48 @@ int32_t epid_nm_stages(epid_ctx* ctx, const epid_batch* frames, int32_t bin, dou
  * of each row, and mask: a new uint8 batch [2n][h][w] whose frame 2k is the eroded binary of frame k. */
 int32_t epid_nm_fov(epid_ctx* ctx, const epid_batch* binary, double erode, struct epid_nm_result* results, epid_batch** mask);
 
+/* pylinac.nuclear.TomographicContrast (nuclear.py:1553-1856) on uint16 SPECT volumes, bit-identical to the reference.  A batch of
+ * volumes is a uint16 batch of n = volumes x nz slices, volume v being slices v * nz .. v * nz + nz - 1.  The rows are plain structs
+ * (not typedefs): their layouts are checked by tests/test_tomo_contrast_host.py. */
+enum { EPID_NT_OK = 0, EPID_NT_NO_COMPONENT = 1 /* no pixel at or above 10 % of the volume's maximum: slice_data skips the slice */ };
+struct epid_nt_slice { /* one per slice: slice_data (nuclear.py:1620-1651) before the area filter */
+    int32_t status;
+    int32_t longest;                   /* longest bounding-box side of the largest 4-connected region (first label on ties) */
+    int32_t erosion;                   /* rint(ufov_erode * longest) */
+    int32_t area;                      /* pixels of the FOV: exact EDT of the whole binary > erosion / 2 */
+    int32_t max, min;                  /* of the FOV pixels (0 when the FOV is empty) */
+    uint64_t sum;                      /* exact sum of the FOV pixels */
+    double centroid_row;               /* the largest region's centroid: exact coordinate sum / area, one rounding */
+    double centroid_col;
+    double uniformity;                 /* michelson of the FOV pixels (nan for an empty FOV) */
+    double value;                      /* their mean (nan for an empty FOV) */
+};
+struct epid_nt_sphere_in { /* one sphere search: minimize(contrast_f, x0, method="Nelder-Mead", bounds=(lb, ub)) (nuclear.py:1714-1724) */
+    double x0[3];                      /* (col, row, z) */
+    double lb[3];
+    double ub[3];
+    double r2;                         /* radius**2 as Python computes it */
+    double baseline;                   /* uniformity_value */
+    int32_t volume;                    /* index of the volume in the batch */
+    int32_t pad;
+};
+struct epid_nt_sphere { /* the search's result and the sphere at res.x */
+    int32_t nfev, nit;
+    int32_t status;                    /* scipy's warnflag: 0 converged, 1 maxfun reached, 2 maxiter reached */
+    int32_t n_empty;                   /* evaluations whose sphere held no voxel ("Mean of empty slice") */
+    int32_t count;                     /* voxels of the sphere at res.x */
+    int32_t min;                       /* their minimum (0 when count is 0) */
+    uint64_t sum;                      /* their exact sum */
+    double x[3];                       /* res.x */
+    double fun;                        /* res.fun */
+};
+/* slice_data's per-slice quantities of every slice (results: host rows [n]); ufov_erode = 1 - ufov_ratio computed by the caller. */
+int32_t epid_nt_slices(epid_ctx* ctx, const epid_batch* volumes, int32_t nz, double ufov_erode, struct epid_nt_slice* results);
+/* nspheres sphere searches (spheres, results: host rows [nspheres]), each scipy 1.18.1's _minimize_neldermead with its default
+ * options, bounds and at most maxfun evaluations and maxiter iterations (minimize() passes 600 for both in 3-D). */
+int32_t epid_nt_spheres(epid_ctx* ctx, const epid_batch* volumes, int32_t nz, const struct epid_nt_sphere_in* spheres, int32_t nspheres,
+                        int32_t maxfun, int32_t maxiter, struct epid_nt_sphere* results);
+
 /* ----------------------------------------------------------------------------------------- multi-GPU (NCCL)
  * The batch shards by frame index with no data-path collective; the only exchange is the final gather of the
  * fixed-size per-frame result structs (SURVEY.md 8e).  id: 128-byte ncclUniqueId created by rank 0. */

@@ -239,6 +239,20 @@ NM_RESULT_DTYPE = np.dtype([
     ("du_max", "<f8", (4,))], align=True)
 
 
+NT_OK, NT_NO_COMPONENT = 0, 1
+
+NT_SLICE_DTYPE = np.dtype([
+    ("status", "<i4"), ("longest", "<i4"), ("erosion", "<i4"), ("area", "<i4"), ("max", "<i4"), ("min", "<i4"), ("sum", "<u8"),
+    ("centroid_row", "<f8"), ("centroid_col", "<f8"), ("uniformity", "<f8"), ("value", "<f8")], align=True)
+
+NT_SPHERE_IN_DTYPE = np.dtype([("x0", "<f8", (3,)), ("lb", "<f8", (3,)), ("ub", "<f8", (3,)), ("r2", "<f8"), ("baseline", "<f8"),
+                               ("volume", "<i4"), ("pad", "<i4")], align=True)
+
+NT_SPHERE_DTYPE = np.dtype([
+    ("nfev", "<i4"), ("nit", "<i4"), ("status", "<i4"), ("n_empty", "<i4"), ("count", "<i4"), ("min", "<i4"), ("sum", "<u8"),
+    ("x", "<f8", (3,)), ("fun", "<f8")], align=True)
+
+
 REGION_DTYPE = np.dtype([("threshold_index", "<i4"), ("label_root", "<i4"), ("bbox", "<i4", (4,)), ("area", "<f8"), ("area_filled", "<f8"),
                          ("perimeter", "<f8"), ("equivalent_diameter", "<f8"), ("centroid_y", "<f8"), ("centroid_x", "<f8"),
                          ("wcentroid_y", "<f8"), ("wcentroid_x", "<f8")], align=True)
@@ -312,6 +326,8 @@ _SIGNATURES = {
     "epid_nm_uniformity": [_P, _P, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_double, _P, C.POINTER(_P), C.POINTER(_P)],
     "epid_nm_stages": [_P, _P, C.c_int32, C.c_double, C.c_double, C.c_int32, C.c_double, _P, _P, _P, _P, _P],
     "epid_nm_fov": [_P, _P, C.c_double, _P, C.POINTER(_P)],
+    "epid_nt_slices": [_P, _P, C.c_int32, C.c_double, _P],
+    "epid_nt_spheres": [_P, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P],
     "epid_canny": [_P, _P, _P, C.c_int32, C.c_double, C.c_double, C.POINTER(_P)],
     "epid_hough_line": [_P, _P, C.c_int32, _P, C.POINTER(_P), C.POINTER(C.c_int32)],
     "epid_hough_candidates": [_P, _P, C.c_int32, C.c_int32, C.c_double, C.c_int32, _P, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
@@ -960,6 +976,31 @@ def nm_fov(ctx: Context, binary: np.ndarray, erode: float) -> tuple[np.ndarray, 
         with Batch(ctx, h) as m:
             mask = m.download()[0]
     return res[0], mask
+
+
+def nt_slices(ctx: Context, volumes, nz: int, ufov_erode: float) -> np.ndarray:
+    """epid_nt_slices on uint16 volumes (Batch of n x nz slices, or ndarray [n, nz, h, w]) -> one NT_SLICE_DTYPE row per slice,
+    [n * nz]"""
+    if not isinstance(volumes, Batch):
+        volumes = np.ascontiguousarray(volumes).reshape(-1, *np.shape(volumes)[-2:])
+    with batch_for(ctx, volumes, np.uint16) as b:
+        (n, _, _), _ = b.shape_dtype
+        res = np.zeros(n, NT_SLICE_DTYPE)
+        _unsupported_as_not_implemented(lib().epid_nt_slices(ctx.handle, b.handle, int(nz), float(ufov_erode), _ptr(res)))
+    return res
+
+
+def nt_spheres(ctx: Context, volumes, nz: int, spheres: np.ndarray, maxfun: int = 600, maxiter: int = 600) -> np.ndarray:
+    """epid_nt_spheres: the sphere searches of `spheres` (NT_SPHERE_IN_DTYPE rows) in uint16 volumes (Batch of n x nz slices, or
+    ndarray [n, nz, h, w]) -> one NT_SPHERE_DTYPE row per sphere"""
+    if not isinstance(volumes, Batch):
+        volumes = np.ascontiguousarray(volumes).reshape(-1, *np.shape(volumes)[-2:])
+    spheres = np.ascontiguousarray(spheres, NT_SPHERE_IN_DTYPE)
+    with batch_for(ctx, volumes, np.uint16) as b:
+        res = np.zeros(len(spheres), NT_SPHERE_DTYPE)
+        _unsupported_as_not_implemented(lib().epid_nt_spheres(ctx.handle, b.handle, int(nz), _ptr(spheres), len(spheres), int(maxfun),
+                                                              int(maxiter), _ptr(res)))
+    return res
 
 
 def divide(ctx: Context, num, den, sign_off=None) -> np.ndarray:

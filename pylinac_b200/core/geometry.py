@@ -208,3 +208,10 @@ class Rectangle:
     @property
     def bl_corner(self) -> Point:
         return self.vertices[3]
+
+
+def direction_to_coords(start_x: float, start_y: float, distance: float, angle_degrees: float) -> tuple[float, float]:
+    """core/geometry.py:43-67: the point `distance` from (start_x, start_y) at `angle_degrees` (0 pointing right, i.e. the unit
+    circle)"""
+    angle_radians = math.radians(angle_degrees)
+    return start_x + distance * math.cos(angle_radians), start_y + distance * math.sin(angle_radians)

@@ -12,6 +12,7 @@
 // and the EDT comparison are evaluated on exact integers and round once, as numpy does.
 #include "ccl.cuh"
 #include "common.cuh"
+#include "nuclear_reduce.cuh"
 
 #include <climits>
 #include <cmath>
@@ -19,37 +20,13 @@
 namespace epid {
 namespace {
 
+using namespace nm;
+
 constexpr int NM_BIN_THREADS = 256;
 constexpr int NM_BIN_COLS = 2048;      // raw columns per pass of k_nm_bin (a multiple of every supported bin)
 constexpr int NM_THREADS = 512;
 constexpr int NM_MAX_BIN = 64;         // 16 * 65535 * 64^2 < 2^32: S stays a uint32
 constexpr int NM_BIG = 1 << 20;        // column distance of a pixel with no background above / below it
-
-struct OpMax {
-    template <class T>
-    __device__ T operator()(T a, T b) const { return a > b ? a : b; }
-};
-struct OpMin {
-    template <class T>
-    __device__ T operator()(T a, T b) const { return a < b ? a : b; }
-};
-struct OpSum {
-    template <class T>
-    __device__ T operator()(T a, T b) const { return a + b; }
-};
-
-// block-wide reduction of a 64-bit value; every thread gets the result
-template <class T, class Op>
-__device__ T block_reduce(T v, Op op, unsigned long long* red) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v = op(v, (T)__shfl_xor_sync(0xffffffffu, (unsigned long long)v, o));
-    __syncthreads();                                        // red[] may still be read by the previous reduction
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = (unsigned long long)v;
-    __syncthreads();
-    T r = (T)red[0];
-    for (int k = 1; k < (int)(blockDim.x >> 5); k++) r = op(r, (T)red[k]);
-    return r;
-}
 
 // block sums of bin x bin raw pixels for binned row blockIdx.x of frame blockIdx.y.  Each thread sums raw columns over the bin's rows
 // (coalesced along the row), then each binned column adds its bin column sums.  VEC: w % 8 == 0, 16-byte loads of 8 pixels.

@@ -1,20 +1,27 @@
-"""pylinac.nuclear (nuclear.py:39-500): MaxCountRate and PlanarUniformity of gamma-camera NM files.
+"""pylinac.nuclear (nuclear.py:39-500, 1553-1856): MaxCountRate, PlanarUniformity and TomographicContrast of gamma-camera NM files.
 
 PlanarUniformity's whole frame pipeline (binning, the NEMA 9-point filter, the threshold, the stray-pixel clean-up, the largest
 component, both FOV erosions, integral and differential uniformity) runs in one device call per batch (csrc/nuclear.cu), bit-identical
 to the reference.  The cleaned frames and FOV masks stay on the device until an attribute needs them.  MaxCountRate takes its exact
-frame sums from epid_frame_stats.  The other nuclear tests are not ported yet (DESIGN.md section 6).
+frame sums from epid_frame_stats.  TomographicContrast makes one device call for the slice analysis of a batch of SPECT volumes and
+one for all its sphere searches (csrc/nuclear_tomo.cu), bit-identical to the reference.  The other nuclear tests are not ported yet
+(DESIGN.md section 6).
 """
 from __future__ import annotations
 
 import json
+import math
+import warnings
 from collections.abc import Sequence
+from functools import cached_property
 from pathlib import Path
+from typing import TypedDict
 
 import numpy as np
 from pydantic import BaseModel
 
 from . import _native as nat
+from .core.geometry import Point, direction_to_coords
 from .core.image import NMImageStack
 from .core.utilities import ResultBase, ResultsDataMixin
 from .core.warnings import capture_warnings
@@ -360,3 +367,307 @@ class MaxCountRate(ResultsDataMixin[MaxCountRateResults]):
     def _generate_results_data(self) -> MaxCountRateResults:
         return MaxCountRateResults(max_countrate=self.max_countrate, frame_duration=self.frame_duration, max_frame=self.max_frame,
                                    sums=self.sums)
+
+
+# ---------------------------------------------------------------------------------------------------- TomographicContrast
+_EMPTY_MEAN = "Mean of empty slice"
+_ALL_NAN_AXIS = "All-NaN axis encountered"
+_BOUNDS_ORDER = "An upper bound is less than the corresponding lower bound."
+
+
+def _michelson(array) -> float:
+    """pylinac.core.contrast.michelson: (max - min) / (max + min), nan values ignored"""
+    l_max, l_min = np.nanmax(array), np.nanmin(array)
+    return (l_max - l_min) / (l_max + l_min)
+
+
+def create_sphere_mask(array_shape: tuple[float, float, float], row: float, col: float, zed: float, radius: float) -> np.ndarray:
+    """A mask of a sphere in an array (nuclear.py:1825-1835)."""
+    z, y, x = np.ogrid[: array_shape[0], : array_shape[1], : array_shape[2]]
+    return (x - col) ** 2 + (y - row) ** 2 + (z - zed) ** 2 <= radius**2
+
+
+def sample_sphere(array: np.ndarray, row: float, col: float, zed: float, radius: float) -> np.ndarray:
+    """A float64 copy of `array` that is nan outside the sphere (nuclear.py:1838-1847)."""
+    sphere_mask = create_sphere_mask(array.shape, row=row, col=col, zed=zed, radius=radius)
+    sphere_sample = np.full(array.shape, np.nan)
+    sphere_sample[sphere_mask] = array[sphere_mask]
+    return sphere_sample
+
+
+def contrast_f(coords: np.ndarray, array: np.ndarray, radius: float, uniformity_baseline: float) -> float:
+    """The objective of the sphere search (nuclear.py:1850-1856): -michelson([sphere mean, baseline]) x 100.  The device runs it
+    on the sphere's bounding box; this host version is the reference's."""
+    col, row, zed = coords
+    sample = sample_sphere(array, col=col, row=row, zed=zed, radius=radius)
+    return -_michelson(np.asarray([np.nanmean(sample), uniformity_baseline])) * 100
+
+
+class TomographicROI:
+    """One sphere at the searched position (nuclear.py:1553-1593).  The analysis gives its exact sum, count and min from the device;
+    built by hand (without `stats`), it samples `array3d` as the reference does.  ``sphere_array`` is built on first access."""
+
+    def __init__(self, array3d: np.ndarray | None, uniformity_baseline: float, x: float, y: float, z: float, radius: float,
+                 number: str | int, stats: tuple[int, int, int] | None = None):
+        self.array3d, self.uniformity_baseline = array3d, uniformity_baseline
+        self.x, self.y, self.z, self.radius, self.number = x, y, z, radius, number
+        self._stats = stats
+
+    @cached_property
+    def sphere_array(self) -> tuple[np.ndarray]:
+        """(the volume as float64, nan outside the sphere,): a 1-tuple, as the reference builds it"""
+        if self.array3d is None:
+            raise RuntimeError("this ROI was analysed from a device batch and keeps no host volume")
+        return (sample_sphere(self.array3d, col=self.x, row=self.y, zed=self.z, radius=self.radius),)
+
+    @property
+    def mean_value(self) -> float:
+        if self._stats is None:
+            return float(np.nanmean(self.sphere_array))
+        s, n, _ = self._stats
+        if n == 0:
+            warnings.warn(_EMPTY_MEAN, RuntimeWarning, stacklevel=2)
+            return math.nan
+        return float(np.float64(s) / np.float64(n))
+
+    @property
+    def min_value(self) -> float:
+        if self._stats is None:
+            return float(np.nanmin(self.sphere_array))
+        if self._stats[1] == 0:
+            warnings.warn(_ALL_NAN_AXIS, RuntimeWarning, stacklevel=2)
+            return math.nan
+        return float(self._stats[2])
+
+    @property
+    def mean_contrast(self) -> float:
+        return _michelson(np.asarray([self.mean_value, self.uniformity_baseline])) * 100
+
+    @property
+    def max_contrast(self) -> float:
+        return _michelson(np.asarray([self.min_value, self.uniformity_baseline])) * 100
+
+
+class TomgraphicSphere(TypedDict):
+    x: float
+    y: float
+    z: float
+    radius: float
+    mean: float
+    mean_contrast: float
+    max_contrast: float
+
+
+class TomographicContrastResults(ResultBase):
+    uniformity_baseline: float  #:
+    spheres: dict[str, TomgraphicSphere]  #:
+
+
+def _slice_data(rows: np.ndarray) -> dict[str, dict]:
+    """slice_data (nuclear.py:1620-1658) from the device rows of one volume's slices: the reference's dict, its warnings for slices
+    with an empty FOV, and its area filter"""
+    uniformities = {}
+    for idx, r in enumerate(rows):
+        if r["status"] == nat.NT_NO_COMPONENT:
+            continue
+        if r["area"] == 0:                    # michelson's nanmax and nanmin, then nanmean, of an all-nan FOV
+            warnings.warn(_ALL_NAN, RuntimeWarning, stacklevel=3)
+            warnings.warn(_ALL_NAN, RuntimeWarning, stacklevel=3)
+            warnings.warn(_EMPTY_MEAN, RuntimeWarning, stacklevel=3)
+        uniformities[str(idx + 1)] = {
+            "fov diameter": int(r["longest"]) - int(r["erosion"]),
+            "center": Point(x=np.float64(r["centroid_col"]), y=np.float64(r["centroid_row"])),
+            "area": int(r["area"]),
+            "uniformity": np.float64(r["uniformity"]),
+            "value": np.float64(r["value"]),
+        }
+    median_area = np.median([v["area"] for v in uniformities.values()])
+    std_area = np.std([v["area"] for v in uniformities.values()])
+    return {k: v for k, v in uniformities.items() if v["area"] > median_area - std_area}
+
+
+class TomographicContrastVolume:
+    """The analysis of one volume of analyze_tomographic_contrast_batch: ``slice_rows`` (the device's NT_SLICE_DTYPE rows),
+    ``slice_data``, ``uniformity_frame``, ``uniformity_value``, ``rois`` and ``searches`` (the NT_SPHERE_DTYPE rows).  A volume with
+    no slice left keeps the reference's ValueError and raises it from ``raise_for_status()`` and every other attribute."""
+
+    def __init__(self, slice_rows: np.ndarray, slice_data: dict):
+        self.slice_rows, self.slice_data = slice_rows, slice_data
+        self.error: Exception | None = None
+        self.searches = np.zeros(0, nat.NT_SPHERE_DTYPE)
+        self._rois: dict[str, TomographicROI] = {}
+
+    def raise_for_status(self) -> None:
+        if self.error is not None:
+            raise self.error
+
+    @property
+    def uniformity_frame(self) -> str:
+        """The frame with the most uniformity."""
+        return min(self.slice_data, key=lambda x: self.slice_data.get(x)["uniformity"])
+
+    @property
+    def uniformity_value(self) -> float:
+        return self.slice_data[self.uniformity_frame]["value"]
+
+    @property
+    def rois(self) -> dict[str, TomographicROI]:
+        self.raise_for_status()
+        return self._rois
+
+
+def _sphere_inputs(out: list[TomographicContrastVolume], pixel_size_mm: float, sphere_diameters_mm, sphere_angles, search_window_px,
+                   search_slices) -> tuple[np.ndarray, list[tuple[int, float]]]:
+    """the host selection (nuclear.py:1693-1712): the NT_SPHERE_IN_DTYPE rows of every sphere search of the volumes of `out`, and
+    each row's (volume, radius).  A volume with no slice left gets the reference's ValueError and no row."""
+    if search_window_px < 0 or search_slices < 0:
+        raise ValueError(_BOUNDS_ORDER)
+    if search_window_px == 0 or search_slices == 0:
+        raise NotImplementedError("a search window of zero fixes a variable, which scipy's minimize handles apart; not supported")
+    spheres, owners = [], []
+    for v, res in enumerate(out):
+        data = res.slice_data
+        if not data:
+            res.error = ValueError(_EMPTY_MAX)
+            continue
+        start = max(data, key=lambda x: data[x]["uniformity"])    # the least uniform slice, usually near the spheres
+        unif, unif_z = data[start], int(start) - 1
+        baseline = res.uniformity_value
+        for angle, diameter in zip(sphere_angles, sphere_diameters_mm):
+            distance = math.sqrt(unif["area"] / math.pi) * 0.65
+            radius = diameter / (2 * pixel_size_mm)
+            col_x, row_y = direction_to_coords(unif["center"].x, unif["center"].y, distance, angle)
+            spheres.append(((col_x, row_y, unif_z), (col_x - search_window_px, row_y - search_window_px, unif_z - search_slices),
+                            (col_x + search_window_px, row_y + search_window_px, unif_z + search_slices), radius**2, baseline, v))
+            owners.append((v, radius))
+    inp = np.zeros(len(spheres), nat.NT_SPHERE_IN_DTYPE)
+    for k, (x0, lb, ub, r2, baseline, v) in enumerate(spheres):
+        inp[k] = (x0, lb, ub, r2, baseline, v, 0)
+    return inp, owners
+
+
+def _search_spheres(ctx, volumes, host, nz: int, out: list[TomographicContrastVolume], pixel_size_mm: float, sphere_diameters_mm,
+                    sphere_angles, search_window_px, search_slices) -> None:
+    """one device call for every sphere search of the volumes of `out`, and their ROIs"""
+    inp, owners = _sphere_inputs(out, pixel_size_mm, sphere_diameters_mm, sphere_angles, search_window_px, search_slices)
+    found = nat.nt_spheres(ctx, volumes, nz, inp, 600, 600)
+    for k, ((v, radius), s) in enumerate(zip(owners, found)):
+        res = out[v]
+        res.searches = np.concatenate([res.searches, found[k:k + 1]])
+        for _ in range(int(s["n_empty"])):
+            warnings.warn(_EMPTY_MEAN, RuntimeWarning, stacklevel=2)
+        col, row, zed = (np.float64(c) for c in s["x"])
+        number = len(res._rois) + 1
+        roi = TomographicROI(None if host is None else host[v], res.uniformity_value, col, row, zed, radius, number,
+                             stats=(int(s["sum"]), int(s["count"]), int(s["min"])))
+        roi._search = s                       # the device row: nfev, nit, status, n_empty, res.fun
+        res._rois[str(number)] = roi
+
+
+def analyze_tomographic_contrast_batch(volumes, pixel_size_mm: float, sphere_diameters_mm: Sequence[float] = (38, 31.8, 25.4, 19.1, 15.9, 12.7),
+                                       sphere_angles: Sequence[float] = (-10, -70, -130, -190, 110, 50), ufov_ratio: float = 0.8,
+                                       search_window_px: int = 5, search_slices: int = 3, *, slices_per_volume: int | None = None,
+                                       device: int | None = None) -> list[TomographicContrastVolume]:
+    """``TomographicContrast.analyze`` for every volume of `volumes`: a uint16 [n, z, h, w] (or [z, h, w]) ndarray, uint8 widened on
+    the host, or a device Batch of n x z slices with ``slices_per_volume=z``.  One device call analyses every slice, the host selects
+    the slices in the reference's own expressions, and one device call runs every sphere search.  Mismatched diameters and angles
+    raise ValueError after the slice stage, as in the reference."""
+    if isinstance(volumes, nat.Batch):
+        (n, h, w), dt = volumes.shape_dtype
+        if dt != np.uint16:
+            raise NotImplementedError(f"nuclear frames of dtype {np.dtype(dt).name} are not supported (uint8 or uint16)")
+        if slices_per_volume is None or slices_per_volume < 1 or n % slices_per_volume:
+            raise ValueError(f"slices_per_volume must divide the batch's {n} slices, got {slices_per_volume}")
+        nz, host = int(slices_per_volume), None
+    else:
+        a = np.asarray(volumes)
+        if a.dtype == np.uint8:
+            a = a.astype(np.uint16)
+        elif a.dtype != np.uint16:
+            raise NotImplementedError(f"nuclear frames of dtype {a.dtype.name} are not supported (uint8 or uint16)")
+        if a.ndim not in (3, 4):
+            raise ValueError(f"volumes must be [n, z, h, w] or [z, h, w], got {a.ndim}-D")
+        host = a[None] if a.ndim == 3 else a
+        nz = host.shape[1]
+        volumes = host
+    ctx = nat.Context.default(device)
+    rows = nat.nt_slices(ctx, volumes, nz, 1 - ufov_ratio)
+    out = [TomographicContrastVolume(r, _slice_data(r)) for r in rows.reshape(-1, nz)]
+    if len(sphere_diameters_mm) != len(sphere_angles):
+        raise ValueError("The number of sphere diameters and angles must be the same.")
+    _search_spheres(ctx, volumes, host, nz, out, pixel_size_mm, sphere_diameters_mm, sphere_angles, search_window_px, search_slices)
+    return out
+
+
+@capture_warnings
+class TomographicContrast(ResultsDataMixin[TomographicContrastResults]):
+    """Sphere contrast of a reconstructed SPECT volume, such as a Jaszczak phantom (nuclear.py:1606-1822)."""
+
+    rois: dict[str, TomographicROI]
+
+    def __init__(self, path: str | Path):
+        super().__init__()
+        self.stack = NMImageStack(path)
+        self.path = Path(path)
+
+    @cached_property
+    def slice_data(self) -> dict[str, dict[str, float | Point]]:
+        """per kept slice (1-based key): its FOV diameter, center, area, uniformity and mean value"""
+        if "ufov_ratio" in self.__dict__:
+            return _slice_data(nat.nt_slices(nat.Context.default(), self._volume(), len(self.stack.frames), 1 - self.ufov_ratio))
+        # before analyze(): the reference reads ufov_ratio at the first slice with a component, so a volume without one gives {}
+        rows = nat.nt_slices(nat.Context.default(), self._volume(), len(self.stack.frames), 0.0)
+        if np.any(rows["status"] == nat.NT_OK):
+            return self.ufov_ratio
+        return _slice_data(rows)
+
+    def _volume(self) -> np.ndarray:
+        a = self.stack._pixels
+        if a.dtype == np.uint8:
+            return a.astype(np.uint16)
+        if a.dtype != np.uint16:
+            raise NotImplementedError(f"nuclear frames of dtype {a.dtype.name} are not supported (uint8 or uint16)")
+        return a
+
+    @property
+    def uniformity_frame(self) -> str:
+        """The frame with the most uniformity."""
+        return min(self.slice_data, key=lambda x: self.slice_data.get(x)["uniformity"])
+
+    @property
+    def uniformity_value(self) -> float:
+        return self.slice_data[self.uniformity_frame]["value"]
+
+    def analyze(self, sphere_diameters_mm: Sequence[float] = (38, 31.8, 25.4, 19.1, 15.9, 12.7),
+                sphere_angles: Sequence[float] = (-10, -70, -130, -190, 110, 50), ufov_ratio: float = 0.8, search_window_px: int = 5,
+                search_slices: int = 3) -> None:
+        """Find each sphere (`sphere_diameters_mm`, at `sphere_angles` degrees) within `search_window_px` pixels and `search_slices`
+        slices of its nominal position by a bounded Nelder-Mead search for the best contrast against the most uniform slice."""
+        self.ufov_ratio = ufov_ratio
+        data = self.slice_data
+        if len(sphere_diameters_mm) != len(sphere_angles):
+            raise ValueError("The number of sphere diameters and angles must be the same.")
+        if not data:
+            raise ValueError(_EMPTY_MAX)
+        res = TomographicContrastVolume(None, data)
+        volume = self._volume()
+        _search_spheres(nat.Context.default(), volume, volume[None], len(volume), [res], float(self.stack.metadata.PixelSpacing[0]),
+                        sphere_diameters_mm, sphere_angles, search_window_px, search_slices)
+        self.rois = res.rois
+
+    def results(self) -> str:
+        """Return a string representation of the results."""
+        s = f"Tomographic Contrast results for {self.path.name}\n"
+        s += f"Uniformity baseline: {self.uniformity_value:.1f}\n"
+        for idx, roi in self.rois.items():
+            s += (f"Sphere {idx}: X={roi.x:.2f},Y={roi.y:.2f},Z={roi.z:.2f} Mean: {roi.mean_value:.2f}; "
+                  f"Mean Contrast: {roi.mean_contrast:.2f}; Max Contrast: {roi.max_contrast:.2f}\n")
+        return s
+
+    def _generate_results_data(self) -> TomographicContrastResults:
+        return TomographicContrastResults(
+            uniformity_baseline=self.uniformity_value,
+            spheres={idx: TomgraphicSphere(x=roi.x, y=roi.y, z=roi.z, radius=roi.radius, mean=roi.mean_value,
+                                           mean_contrast=roi.mean_contrast, max_contrast=roi.max_contrast)
+                     for idx, roi in self.rois.items()},
+        )
