@@ -837,6 +837,42 @@ int32_t epid_nt_slices(epid_ctx* ctx, const epid_batch* volumes, int32_t nz, dou
 int32_t epid_nt_spheres(epid_ctx* ctx, const epid_batch* volumes, int32_t nz, const struct epid_nt_sphere_in* spheres, int32_t nspheres,
                         int32_t maxfun, int32_t maxiter, struct epid_nt_sphere* results);
 
+/* pylinac.nuclear.TomographicUniformity (nuclear.py:1370-1551) on uint16 SPECT volumes, bit-identical to the reference.  A batch of
+ * volumes is a uint16 batch of n = volumes x nz slices, as for epid_nt_slices.  Per volume: the mean m = T / count of the slab of
+ * slices first .. first + count - 1 (T the exact integer sum), then epid_nm_uniformity's pipeline on that float64 frame with every sum
+ * in numpy's / scipy's order, three FOVs (0 UFOV, 1 CFOV, 2 center; erosion k = rint(erode[k] * L) with erode = 1 - size computed by
+ * the caller) and the sums of center_border_ratio.  du_* are indexed [2 * fov + axis].  The row is a plain struct (not a typedef):
+ * its layout is checked by tests/test_tomo_uniformity_host.py.  status takes the EPID_NM_* values. */
+struct epid_tu_result { /* one per volume */
+    int32_t status;
+    int32_t longest;                   /* L */
+    int32_t erosion[3];
+    int32_t n_fov[3];                  /* non-zero FOV pixels (0: integral_uniformity raises) */
+    int32_t max_index[3];              /* first raster index (row * wb + col) of the FOV maximum / minimum */
+    int32_t min_index[3];
+    int32_t du_count[6];               /* windows holding a FOV pixel; the others are all-nan windows */
+    int32_t du_index[6];               /* first (i, j) in row-major order of du_max, as i * wb + j */
+    int32_t center_count;              /* non-zero pixels of the center FOV */
+    int32_t ring_count;                /* non-zero pixels of the UFOV outside the CFOV */
+    double threshold;                  /* the absolute threshold (nan when no value exceeds 10 % of the max) */
+    double iu[3];                      /* integral uniformity, % */
+    double du_max[6];                  /* maximum window uniformity, % */
+    double center_sum;                 /* np.sum of the frame, zero outside those pixels */
+    double ring_sum;
+};
+/* bin: a power of two up to 64; window >= 1; 0 <= first, 1 <= count, first + count <= nz.  results: host rows [volumes].  mean,
+ * cleaned, masks (each may be NULL): new batches, float64 [volumes][h][w] (the slab mean), float64 [volumes][hb][wb] (the reference's
+ * binned_frame) and uint8 [3 x volumes][hb][wb] (the three masks of volume k at 3k .. 3k + 2). */
+int32_t epid_tu_uniformity(epid_ctx* ctx, const epid_batch* volumes, int32_t nz, int32_t first, int32_t count, int32_t bin,
+                           double ufov_erode, double cfov_erode, double center_erode, int32_t window, double threshold,
+                           struct epid_tu_result* results, epid_batch** mean, epid_batch** cleaned, epid_batch** masks);
+/* Diagnostic read-back: the launch sequence of epid_tu_uniformity and host planes of the mean [volumes][h][w], the binned, filtered and
+ * cleaned frames [volumes][hb][wb], the squared EDT (-1 for a frame without a component) and the masks [volumes][3][hb][wb]. */
+int32_t epid_tu_stages(epid_ctx* ctx, const epid_batch* volumes, int32_t nz, int32_t first, int32_t count, int32_t bin,
+                       double ufov_erode, double cfov_erode, double center_erode, int32_t window, double threshold,
+                       struct epid_tu_result* results, double* mean, double* binned, double* filtered, double* cleaned, int32_t* edt2,
+                       uint8_t* masks);
+
 /* ----------------------------------------------------------------------------------------- multi-GPU (NCCL)
  * The batch shards by frame index with no data-path collective; the only exchange is the final gather of the
  * fixed-size per-frame result structs (SURVEY.md 8e).  id: 128-byte ncclUniqueId created by rank 0. */

@@ -253,6 +253,12 @@ NT_SPHERE_DTYPE = np.dtype([
     ("x", "<f8", (3,)), ("fun", "<f8")], align=True)
 
 
+TU_RESULT_DTYPE = np.dtype([
+    ("status", "<i4"), ("longest", "<i4"), ("erosion", "<i4", (3,)), ("n_fov", "<i4", (3,)), ("max_index", "<i4", (3,)),
+    ("min_index", "<i4", (3,)), ("du_count", "<i4", (6,)), ("du_index", "<i4", (6,)), ("center_count", "<i4"), ("ring_count", "<i4"),
+    ("threshold", "<f8"), ("iu", "<f8", (3,)), ("du_max", "<f8", (6,)), ("center_sum", "<f8"), ("ring_sum", "<f8")], align=True)
+
+
 REGION_DTYPE = np.dtype([("threshold_index", "<i4"), ("label_root", "<i4"), ("bbox", "<i4", (4,)), ("area", "<f8"), ("area_filled", "<f8"),
                          ("perimeter", "<f8"), ("equivalent_diameter", "<f8"), ("centroid_y", "<f8"), ("centroid_x", "<f8"),
                          ("wcentroid_y", "<f8"), ("wcentroid_x", "<f8")], align=True)
@@ -328,6 +334,10 @@ _SIGNATURES = {
     "epid_nm_fov": [_P, _P, C.c_double, _P, C.POINTER(_P)],
     "epid_nt_slices": [_P, _P, C.c_int32, C.c_double, _P],
     "epid_nt_spheres": [_P, _P, C.c_int32, _P, C.c_int32, C.c_int32, C.c_int32, _P],
+    "epid_tu_uniformity": [_P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_int32,
+                           C.c_double, _P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)],
+    "epid_tu_stages": [_P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_int32, C.c_double,
+                       _P, _P, _P, _P, _P, _P, _P],
     "epid_canny": [_P, _P, _P, C.c_int32, C.c_double, C.c_double, C.POINTER(_P)],
     "epid_hough_line": [_P, _P, C.c_int32, _P, C.POINTER(_P), C.POINTER(C.c_int32)],
     "epid_hough_candidates": [_P, _P, C.c_int32, C.c_int32, C.c_double, C.c_int32, _P, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
@@ -1001,6 +1011,47 @@ def nt_spheres(ctx: Context, volumes, nz: int, spheres: np.ndarray, maxfun: int 
         _unsupported_as_not_implemented(lib().epid_nt_spheres(ctx.handle, b.handle, int(nz), _ptr(spheres), len(spheres), int(maxfun),
                                                               int(maxiter), _ptr(res)))
     return res
+
+
+def _volume_batch(volumes):
+    """[n, nz, h, w] ndarray volumes as n x nz slices; a Batch as is"""
+    if isinstance(volumes, Batch):
+        return volumes
+    return np.ascontiguousarray(volumes).reshape(-1, *np.shape(volumes)[-2:])
+
+
+def tu_uniformity(ctx: Context, volumes, nz: int, first: int, count: int, bin_size: int, erode, window: int, threshold: float,
+                  arrays: bool = True):
+    """epid_tu_uniformity on uint16 volumes (Batch of n x nz slices, or ndarray [n, nz, h, w]) with the slab [first, first + count) and
+    erode = (UFOV, CFOV, center) 1 - size -> (TU_RESULT_DTYPE rows, mean, cleaned, masks): device Batches of the float64 slab means
+    [n, h, w], the float64 cleaned frames [n, hb, wb] and the uint8 masks [3n, hb, wb], all None when not `arrays`."""
+    with batch_for(ctx, _volume_batch(volumes), np.uint16) as b:
+        (n, _, _), _ = b.shape_dtype
+        res = np.zeros(n // int(nz), TU_RESULT_DTYPE)
+        hs = [_P(), _P(), _P()]
+        _unsupported_as_not_implemented(lib().epid_tu_uniformity(
+            ctx.handle, b.handle, int(nz), int(first), int(count), int(bin_size), *(float(e) for e in erode), int(window),
+            float(threshold), _ptr(res), *(C.byref(h) if arrays else None for h in hs)))
+    if not arrays:
+        return res, None, None, None
+    return (res, *(Batch(ctx, h) for h in hs))
+
+
+def tu_stages(ctx: Context, volumes, nz: int, first: int, count: int, bin_size: int, erode, window: int, threshold: float) -> dict:
+    """Diagnostic read-back of epid_tu_stages: {"results", "mean" [n, h, w], "binned", "filtered", "cleaned" (float64 [n, hb, wb]),
+    "edt2" (int32 squared EDT, -1 for a volume without a component), "masks" (uint8 [n, 3, hb, wb])}."""
+    with batch_for(ctx, _volume_batch(volumes), np.uint16) as b:
+        (n, h, w), _ = b.shape_dtype
+        nv = n // int(nz)
+        hb, wb = -(-h // int(bin_size)), -(-w // int(bin_size))
+        res = np.zeros(nv, TU_RESULT_DTYPE)
+        out = {"mean": np.empty((nv, h, w)), "binned": np.empty((nv, hb, wb)), "filtered": np.empty((nv, hb, wb)),
+               "cleaned": np.empty((nv, hb, wb)), "edt2": np.empty((nv, hb, wb), np.int32), "masks": np.empty((nv, 3, hb, wb), np.uint8)}
+        _unsupported_as_not_implemented(lib().epid_tu_stages(
+            ctx.handle, b.handle, int(nz), int(first), int(count), int(bin_size), *(float(e) for e in erode), int(window),
+            float(threshold), _ptr(res), *(_ptr(a) for a in out.values())))
+    out["results"] = res
+    return out
 
 
 def divide(ctx: Context, num, den, sign_off=None) -> np.ndarray:

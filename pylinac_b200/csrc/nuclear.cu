@@ -12,7 +12,7 @@
 // and the EDT comparison are evaluated on exact integers and round once, as numpy does.
 #include "ccl.cuh"
 #include "common.cuh"
-#include "nuclear_reduce.cuh"
+#include "nuclear_stages.cuh"
 
 #include <climits>
 #include <cmath>
@@ -26,7 +26,6 @@ constexpr int NM_BIN_THREADS = 256;
 constexpr int NM_BIN_COLS = 2048;      // raw columns per pass of k_nm_bin (a multiple of every supported bin)
 constexpr int NM_THREADS = 512;
 constexpr int NM_MAX_BIN = 64;         // 16 * 65535 * 64^2 < 2^32: S stays a uint32
-constexpr int NM_BIG = 1 << 20;        // column distance of a pixel with no background above / below it
 
 // block sums of bin x bin raw pixels for binned row blockIdx.x of frame blockIdx.y.  Each thread sums raw columns over the bin's rows
 // (coalesced along the row), then each binned column adds its bin column sums.  VEC: w % 8 == 0, 16-byte loads of 8 pixels.
@@ -149,167 +148,22 @@ __global__ void __launch_bounds__(NM_THREADS) k_nm_frame(const TIn* __restrict__
     }
     __syncthreads();
 
-    // ---- 4-connected labelling: roots are the smallest index of their component (skimage's raster label order)
-    for (int p = tid; p < N; p += nt) {
-        if (P[p] < 0) continue;
-        const int i = p / wb, j = p - i * wb;
-        if (j > 0 && P[p - 1] >= 0) gl_union(P, p, p - 1);
-        if (i > 0 && P[p - wb] >= 0) gl_union(P, p, p - wb);
-    }
-    __syncthreads();
-    for (int p = tid; p < N; p += nt) {
-        A[p] = 0;
-        if (P[p] >= 0) P[p] = gl_find(P, p);
-    }
-    __syncthreads();
-    for (int p = tid; p < N; p += nt)
-        if (P[p] >= 0) atomicAdd(&A[P[p]], 1);
-    __syncthreads();
-    // largest area; on ties the lowest label, i.e. the smallest root index
-    unsigned long long key = 0;
-    for (int p = tid; p < N; p += nt) {
-        if (P[p] != p) continue;
-        const unsigned long long k = ((unsigned long long)A[p] << 32) | (0xffffffffu - (uint32_t)p);
-        key = k > key ? k : key;
-    }
-    key = block_reduce(key, OpMax(), red);
-    if (key == 0) {               // no component: get_fov's max() over no regions raises
+    label_areas(P, A, hb, wb);
+    const int longest = largest_longest(P, A, hb, wb, red);
+    if (longest == 0) {           // no component: get_fov's max() over no regions raises
         if (tid == 0) {
             r.status = EPID_NM_NO_COMPONENT;
             res[f] = r;
         }
         return;
     }
-    const int root = (int)(0xffffffffu - (uint32_t)key);
-    long long rmin = LLONG_MAX, rmax = -1, cmin = LLONG_MAX, cmax = -1;
-    for (int p = tid; p < N; p += nt) {
-        if (P[p] != root) continue;
-        const int i = p / wb, j = p - i * wb;
-        rmin = min(rmin, (long long)i);
-        rmax = max(rmax, (long long)i);
-        cmin = min(cmin, (long long)j);
-        cmax = max(cmax, (long long)j);
-    }
-    rmin = block_reduce(rmin, OpMin(), red);
-    rmax = block_reduce(rmax, OpMax(), red);
-    cmin = block_reduce(cmin, OpMin(), red);
-    cmax = block_reduce(cmax, OpMax(), red);
-    const int longest = (int)max(rmax - rmin + 1, cmax - cmin + 1);
     // int(round((1 - size) * longest)): Python rounds halves to even, as rint does
     const int eu = (int)rint(ufov_erode * (double)longest), ec = (int)rint(cfov_erode * (double)longest);
     r.longest = longest;
     r.erosion[0] = eu;
     r.erosion[1] = ec;
-
-    // ---- exact squared EDT of the whole binary frame: column distances, then the row-wise minimum of dk^2 + g^2
-    for (int j = tid; j < wb; j += nt) {
-        int g = NM_BIG;
-        for (int i = 0; i < hb; i++) {
-            const int p = i * wb + j;
-            g = P[p] >= 0 ? min(g + 1, NM_BIG) : 0;
-            A[p] = g;
-        }
-        g = NM_BIG;
-        for (int i = hb - 1; i >= 0; i--) {
-            const int p = i * wb + j;
-            g = P[p] >= 0 ? min(g + 1, NM_BIG) : 0;
-            A[p] = min(A[p], g);
-        }
-    }
-    __syncthreads();
-    for (int p = tid; p < N; p += nt) {      // each thread reads and writes only its own P[p]
-        if (P[p] < 0) {
-            P[p] = 0;
-        } else {
-            const int i = p / wb, j = p - i * wb;
-            const int* g = A + (size_t)i * wb;
-            long long best = (long long)g[j] * g[j];
-            for (int k = 1; (long long)k * k < best && (j - k >= 0 || j + k < wb); k++) {
-                if (j - k >= 0) best = min(best, (long long)k * k + (long long)g[j - k] * g[j - k]);
-                if (j + k < wb) best = min(best, (long long)k * k + (long long)g[j + k] * g[j + k]);
-            }
-            P[p] = (int)min(best, (long long)INT_MAX);
-        }
-        if (out.edt2) out.edt2[fo + p] = P[p];
-    }
-    __syncthreads();
-
-    // ---- FOV masks: distance > erosion / 2  <=>  4 d^2 > erosion^2 (every pixel when the erosion is negative)
-    const long long e2[2] = {(long long)eu * eu, (long long)ec * ec};
-    const bool all[2] = {eu < 0, ec < 0};
-    auto in_fov = [&](int p, int k) { return all[k] || 4LL * P[p] > e2[k]; };
-    unsigned long long mxk[2] = {0, 0}, mnk[2] = {~0ull, ~0ull}, nfov[2] = {0, 0};
-    for (int p = tid; p < N; p += nt) {
-        for (int k = 0; k < 2; k++) {
-            const bool m = in_fov(p, k);
-            if (out.masks) out.masks[(2 * (size_t)f + k) * N + p] = m;
-            if (!m || S[p] == 0) continue;
-            const unsigned long long hi = (unsigned long long)S[p] << 32;
-            mxk[k] = max(mxk[k], hi | (0xffffffffu - (uint32_t)p));   // max value, first index
-            mnk[k] = min(mnk[k], hi | (uint32_t)p);                    // min value, first index
-            nfov[k]++;
-        }
-    }
-    for (int k = 0; k < 2; k++) {
-        mxk[k] = block_reduce(mxk[k], OpMax(), red);
-        mnk[k] = block_reduce(mnk[k], OpMin(), red);
-        nfov[k] = block_reduce(nfov[k], OpSum(), red);
-        r.n_fov[k] = (int)nfov[k];
-        if (nfov[k]) {
-            const unsigned long long smx = mxk[k] >> 32, smn = mnk[k] >> 32;
-            r.max_index[k] = (int)(0xffffffffu - (uint32_t)mxk[k]);
-            r.min_index[k] = (int)(uint32_t)mnk[k];
-            r.iu[k] = (double)(smx - smn) / (double)(smx + smn) * 100.0;   // michelson(S / 16) * 100: the 1/16 cancels exactly
-        }
-    }
-
-    // ---- differential uniformity: windows of `win` pixels along axis 0 (a = 0) and axis 1 (a = 1) over the non-zero FOV pixels; a
-    // window counts when it holds at least one.  Per (FOV, axis): the max of the x100 values and its first (i, j) in row-major order.
-    for (int k = 0; k < 2; k++) {
-        for (int a = 0; a < 2; a++) {
-            const int ni = a == 0 ? hb - win + 1 : hb, nj = a == 0 ? wb : wb - win + 1;
-            const int step = a == 0 ? wb : 1;
-            const long long npos = ni > 0 && nj > 0 ? (long long)ni * nj : 0;
-            unsigned long long vbest = 0, cnt = 0;
-            for (long long q = tid; q < npos; q += nt) {
-                const int i = (int)(q / nj), j = (int)(q - (long long)i * nj);
-                uint32_t mx = 0, mn = UINT_MAX;
-                for (int t = 0, p = i * wb + j; t < win; t++, p += step) {
-                    if (!in_fov(p, k) || S[p] == 0) continue;
-                    mx = max(mx, S[p]);
-                    mn = min(mn, S[p]);
-                }
-                if (mx == 0) continue;
-                const double v = (double)(mx - mn) / (double)((unsigned long long)mx + mn) * 100.0;
-                vbest = max(vbest, (unsigned long long)__double_as_longlong(v));   // v >= 0: the bits order like the values
-                cnt++;
-            }
-            vbest = block_reduce(vbest, OpMax(), red);
-            cnt = block_reduce(cnt, OpSum(), red);
-            unsigned long long pos = ~0ull;
-            for (long long q = tid; q < npos && cnt; q += nt) {
-                const int i = (int)(q / nj), j = (int)(q - (long long)i * nj);
-                uint32_t mx = 0, mn = UINT_MAX;
-                for (int t = 0, p = i * wb + j; t < win; t++, p += step) {
-                    if (!in_fov(p, k) || S[p] == 0) continue;
-                    mx = max(mx, S[p]);
-                    mn = min(mn, S[p]);
-                }
-                if (mx == 0) continue;
-                const double v = (double)(mx - mn) / (double)((unsigned long long)mx + mn) * 100.0;
-                if ((unsigned long long)__double_as_longlong(v) == vbest) {
-                    pos = (unsigned long long)i * wb + j;
-                    break;                                  // q increases, so the thread's first hit is its smallest position
-                }
-            }
-            pos = block_reduce(pos, OpMin(), red);
-            r.du_count[2 * k + a] = (int)cnt;
-            if (cnt) {
-                r.du_max[2 * k + a] = __longlong_as_double((long long)vbest);
-                r.du_index[2 * k + a] = (int)pos;
-            }
-        }
-    }
+    squared_edt(P, A, hb, wb, out.edt2 ? out.edt2 + fo : nullptr);
+    fov_uniformity<2>(S, P, FovMasks<2>(r.erosion), hb, wb, win, out.masks ? out.masks + 2 * fo : nullptr, red, r);
     if (tid == 0) res[f] = r;
 }
 

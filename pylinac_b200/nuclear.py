@@ -1,11 +1,13 @@
-"""pylinac.nuclear (nuclear.py:39-500, 1553-1856): MaxCountRate, PlanarUniformity and TomographicContrast of gamma-camera NM files.
+"""pylinac.nuclear (nuclear.py:39-500, 1370-1856): MaxCountRate, PlanarUniformity, TomographicUniformity and TomographicContrast of
+gamma-camera NM files.
 
 PlanarUniformity's whole frame pipeline (binning, the NEMA 9-point filter, the threshold, the stray-pixel clean-up, the largest
 component, both FOV erosions, integral and differential uniformity) runs in one device call per batch (csrc/nuclear.cu), bit-identical
 to the reference.  The cleaned frames and FOV masks stay on the device until an attribute needs them.  MaxCountRate takes its exact
 frame sums from epid_frame_stats.  TomographicContrast makes one device call for the slice analysis of a batch of SPECT volumes and
-one for all its sphere searches (csrc/nuclear_tomo.cu), bit-identical to the reference.  The other nuclear tests are not ported yet
-(DESIGN.md section 6).
+one for all its sphere searches (csrc/nuclear_tomo.cu), bit-identical to the reference.  TomographicUniformity averages a slab of
+slices and runs the planar pipeline on that float64 frame, with a third (center) FOV, in one device call per batch
+(csrc/nuclear_tu.cu), bit-identical to the reference.  The other nuclear tests are not ported yet (DESIGN.md section 6).
 """
 from __future__ import annotations
 
@@ -79,8 +81,8 @@ def get_fov(array: np.ndarray, size: float) -> tuple[np.ndarray, np.ndarray, np.
 class _DeviceArrays:
     """The cleaned frames and FOV masks of one analyze_batch call, on the device until first read, then downloaded once."""
 
-    def __init__(self, cleaned: nat.Batch | None, masks: nat.Batch | None):
-        self._batches = {"cleaned": cleaned, "masks": masks}
+    def __init__(self, cleaned: nat.Batch | None, masks: nat.Batch | None, mean: nat.Batch | None = None):
+        self._batches = {"cleaned": cleaned, "masks": masks, "mean": mean}
         self._host = {}
 
     def get(self, name: str) -> np.ndarray:
@@ -98,6 +100,8 @@ class FOV:
     arrays are downloaded on first access.  Unlike the reference's dataclass it is built by the analysis from a device row, not from
     a FOV array."""
 
+    _masks_per_frame = 2           # the masks batch holds this many masks per frame, FOV k of frame f at f * _masks_per_frame + k
+
     def __init__(self, name: str, window_size: int, row, k: int, shape: tuple[int, int], arrays: _DeviceArrays, frame: int):
         self.name = name
         self.window_size = window_size
@@ -106,7 +110,7 @@ class FOV:
     @property
     def mask(self) -> np.ndarray:
         """the eroded binary of the frame (bool)"""
-        return self._arrays.get("masks")[2 * self._frame + self._k].astype(bool)
+        return self._arrays.get("masks")[self._masks_per_frame * self._frame + self._k].astype(bool)
 
     @property
     def fov(self) -> np.ndarray:
@@ -367,6 +371,294 @@ class MaxCountRate(ResultsDataMixin[MaxCountRateResults]):
     def _generate_results_data(self) -> MaxCountRateResults:
         return MaxCountRateResults(max_countrate=self.max_countrate, frame_duration=self.frame_duration, max_frame=self.max_frame,
                                    sums=self.sums)
+
+
+# ---------------------------------------------------------------------------------------------------- TomographicUniformity
+_EMPTY_MEAN_DOT = "Mean of empty slice."
+_INVALID_DIVIDE = "invalid value encountered in divide"
+_INVALID_SCALAR_DIVIDE = "invalid value encountered in scalar divide"
+
+
+def _slab(n: int, first_frame: int, last_frame: int) -> tuple[int, int]:
+    """TomographicUniformity.analyze's frame checks, in the reference's expressions and order: the slab [first, last) of n slices,
+    which is empty when last is 0"""
+    if first_frame < 0:
+        raise ValueError("The first frame index is outside the array bounds. Increase the first frame index.")
+    if last_frame < 0:
+        last_frame += n
+    if last_frame >= n:
+        raise ValueError("The last frame index is outside the array bounds. Decrease the last frame index.")
+    if 0 < last_frame <= first_frame:
+        raise ValueError("The first frame index must be less than the last frame index.")
+    return first_frame, last_frame
+
+
+def _warn_empty_slab() -> None:
+    """the warnings of the reference on an empty slab: mean(axis=0) of no slice, then preprocess's mean of an empty selection"""
+    warnings.warn(_EMPTY_MEAN_DOT, RuntimeWarning, stacklevel=3)
+    warnings.warn(_INVALID_DIVIDE, RuntimeWarning, stacklevel=3)
+    _warn_empty_threshold()
+
+
+def _warn_empty_threshold() -> None:
+    """preprocess's ``array[array > max * 0.10].mean()`` of an empty selection"""
+    warnings.warn(_EMPTY_MEAN_DOT, RuntimeWarning, stacklevel=4)
+    warnings.warn(_INVALID_SCALAR_DIVIDE, RuntimeWarning, stacklevel=4)
+
+
+class _SlabFOV(FOV):
+    """A FOV of TomographicUniformity: three masks per volume (UFOV, CFOV, center), and the reference's "All-NaN slice encountered"
+    warnings, two per all-nan window (nanmax, nanmin), emitted from the device row's window counts on the first differential-uniformity
+    access (the reference caches the window loop).  The center FOV's ``fov`` is nan where it is 0, as center_border_ratio leaves it."""
+
+    _masks_per_frame = 3
+
+    def __init__(self, *args, nan_zeros: bool = False, **kwargs):
+        super().__init__(*args, **kwargs)
+        self._nan_zeros = nan_zeros
+        self._windows_done = False
+
+    @property
+    def fov(self) -> np.ndarray:
+        a = super().fov
+        return np.where(a == 0, np.nan, a) if self._nan_zeros else a
+
+    def _axis_max(self, axis: int) -> tuple[float, tuple[int, int]]:
+        if not self._windows_done and not (self.window_size > self._shape[0] or self.window_size > self._shape[1]):
+            self._windows_done = True
+            hb, wb = self._shape
+            totals = ((hb - self.window_size + 1) * wb, hb * (wb - self.window_size + 1))     # the y windows first, then x
+            for a in (0, 1):
+                for _ in range(2 * (totals[a] - int(self._row["du_count"][2 * self._k + a]))):
+                    warnings.warn(_ALL_NAN, RuntimeWarning, stacklevel=4)
+        return super()._axis_max(axis)
+
+
+def _center_border_ratio(row) -> np.float64:
+    """np.nanmean(center) / np.nanmean(ring) from the exact-order sums and counts of the device row"""
+    means = []
+    for key in ("center", "ring"):
+        n = int(row[f"{key}_count"])
+        if n == 0:
+            warnings.warn(_EMPTY_MEAN, RuntimeWarning, stacklevel=3)
+            means.append(np.float64(np.nan))
+        else:
+            means.append(np.float64(row[f"{key}_sum"]) / np.float64(n))
+    return means[0] / means[1]
+
+
+class TomographicUniformityVolume:
+    """One volume of analyze_tomographic_uniformity_batch: ``row`` (the device's TU_RESULT_DTYPE row), ``ufov``, ``cfov`` and
+    ``center_fov`` (FOV), ``center_border_ratio``, ``binned_frame`` (the cleaned float64 frame) and ``mean_frame`` (the slab mean)."""
+
+    def __init__(self, row, window_size: int, shape: tuple[int, int], arrays: _DeviceArrays, volume: int):
+        self.row = row
+        self._arrays, self._volume = arrays, volume
+        self.ufov = _SlabFOV("UFOV", window_size, row, 0, shape, arrays, volume)
+        self.cfov = _SlabFOV("CFOV", window_size, row, 1, shape, arrays, volume)
+        self.center_fov = _SlabFOV("Center", window_size, row, 2, shape, arrays, volume, nan_zeros=True)
+
+    @property
+    def status(self) -> int:
+        return int(self.row["status"])
+
+    def raise_for_status(self) -> None:
+        """get_fov's ValueError for a volume with no component left after the clean-up"""
+        if self.status == nat.NM_NO_COMPONENT:
+            raise ValueError(_EMPTY_MAX)
+
+    @property
+    def center_border_ratio(self) -> np.float64:
+        self.raise_for_status()
+        return _center_border_ratio(self.row)
+
+    @property
+    def binned_frame(self) -> np.ndarray:
+        return self._arrays.get("cleaned")[self._volume]
+
+    @property
+    def mean_frame(self) -> np.ndarray:
+        return self._arrays.get("mean")[self._volume]
+
+
+def _volumes(volumes, slices_per_volume):
+    """(uint16 volumes as an [n, z, h, w] ndarray or a device Batch, z, h, w); uint8 widened, other dtypes NotImplementedError"""
+    if isinstance(volumes, nat.Batch):
+        (n, h, w), dt = volumes.shape_dtype
+        if dt != np.uint16:
+            raise NotImplementedError(f"nuclear frames of dtype {np.dtype(dt).name} are not supported (uint8 or uint16)")
+        if slices_per_volume is None or slices_per_volume < 1 or n % slices_per_volume:
+            raise ValueError(f"slices_per_volume must divide the batch's {n} slices, got {slices_per_volume}")
+        return volumes, int(slices_per_volume), h, w
+    a = np.asarray(volumes)
+    if a.dtype == np.uint8:
+        a = a.astype(np.uint16)
+    elif a.dtype != np.uint16:
+        raise NotImplementedError(f"nuclear frames of dtype {a.dtype.name} are not supported (uint8 or uint16)")
+    if a.ndim not in (3, 4):
+        raise ValueError(f"volumes must be [n, z, h, w] or [z, h, w], got {a.ndim}-D")
+    a = a[None] if a.ndim == 3 else a
+    return a, a.shape[1], a.shape[2], a.shape[3]
+
+
+def analyze_tomographic_uniformity_batch(volumes, pixel_size_mm: float, first_frame: int = 0, last_frame: int = -1,
+                                         ufov_ratio: float = 0.8, cfov_ratio: float = 0.75, center_ratio: float = 0.4,
+                                         threshold: float = 0.75, window_size: int = 5, *, slices_per_volume: int | None = None,
+                                         arrays: bool = True, device: int | None = None) -> list[TomographicUniformityVolume]:
+    """``TomographicUniformity.analyze`` for every volume of `volumes`: a uint16 [n, z, h, w] (or [z, h, w]) ndarray, uint8 widened on
+    the host, or a device Batch of n x z slices with ``slices_per_volume=z``.  The frame checks raise the reference's ValueError before
+    any device call, as does an empty slab (last frame 0).  One device call analyses every volume; `arrays` keeps the slab means,
+    cleaned frames and masks on the device for ``mean_frame`` / ``binned_frame`` / ``fov``."""
+    if int(window_size) != window_size or window_size < 1:
+        raise ValueError(f"window_size must be a positive integer, got {window_size}")
+    volumes, nz, h, w = _volumes(volumes, slices_per_volume)
+    first, last = _slab(nz, first_frame, last_frame)
+    if last == 0:
+        _warn_empty_slab()
+        raise ValueError(_EMPTY_MAX)
+    b = determine_binning(pixel_size_mm)
+    # the reference's own expressions: 1 - size with size = cfov_ratio * ufov_ratio (CFOV) and center_ratio * ufov_ratio (center)
+    erode = (1 - ufov_ratio, 1 - cfov_ratio * ufov_ratio, 1 - center_ratio * ufov_ratio)
+    rows, mean, cleaned, masks = nat.tu_uniformity(nat.Context.default(device), volumes, nz, first, last - first, b, erode,
+                                                   int(window_size), threshold, arrays=arrays)
+    dev = _DeviceArrays(cleaned, masks, mean)
+    shape = (-(-h // b), -(-w // b))
+    return [TomographicUniformityVolume(r, int(window_size), shape, dev, v) for v, r in enumerate(rows)]
+
+
+class _SlabMeanFrame:
+    """stack.frames[0] after TomographicUniformity.analyze: the first frame's header with the slab mean as its array, downloaded from
+    the device on first access"""
+
+    def __init__(self, frame, arrays: _DeviceArrays):
+        self._frame, self._arrays, self._array = frame, arrays, None
+
+    def __getattr__(self, name):
+        return getattr(self._frame, name)
+
+    @property
+    def array(self) -> np.ndarray:
+        if self._array is None:
+            self._array = self._arrays.get("mean")[0]
+        return self._array
+
+    @array.setter
+    def array(self, value: np.ndarray) -> None:
+        self._array = value
+
+
+class TomographicUniformityResults(ResultBase):
+    cfov_integral_uniformity: float
+    cfov_differential_uniformity: float
+    ufov_integral_uniformity: float
+    ufov_differential_uniformity: float
+    center_border_ratio: float
+    first_frame: int
+    last_frame: int
+
+
+@capture_warnings
+class TomographicUniformity(ResultsDataMixin[TomographicUniformityResults], PlanarUniformity):
+    """Tomographic uniformity of a SPECT volume, typically a Jaszczak phantom (nuclear.py:1380-1551): PlanarUniformity's analysis of
+    the mean of a slab of slices, and the center-to-border ratio."""
+
+    center_ratio: float
+    first_frame: int
+    last_frame: int
+    threshold: float
+
+    def __init__(self, path: str | Path) -> None:
+        PlanarUniformity.__init__(self, path)
+
+    @property
+    def frame_result(self) -> dict:
+        """We always have a single result"""
+        return self.frame_results[self.frame_key]
+
+    @property
+    def frame_key(self) -> str:
+        """The key for the single frame result"""
+        return f"{self.first_frame}:{self.last_frame}"
+
+    def center_border_ratio(self, center_ratio: float, window_size: int) -> float:
+        """The center-to-border ratio as defined by the NMQC toolkit: the mean of the center FOV (`center_ratio` of the phantom) over
+        the mean of the border, the UFOV without the CFOV.  Stores the center FOV as ``frame_result["center_fov"]``."""
+        vol = self._analysed
+        if (center_ratio, window_size) != (vol["center"], vol["window"]):
+            res = self._run(vol["first"], vol["last"], vol["ufov"], vol["cfov"], 1 - center_ratio, window_size)
+        else:
+            res = vol["result"]
+        self.frame_result["center_fov"] = res.center_fov
+        return _center_border_ratio(res.row)
+
+    def _run(self, first: int, last: int, ufov_erode: float, cfov_erode: float, center_erode: float, window_size: int):
+        b = determine_binning(float(self.stack.metadata.PixelSpacing[0]))
+        a = self._volume
+        rows, mean, cleaned, masks = nat.tu_uniformity(nat.Context.default(), a[None], len(a), first, last - first, b,
+                                                       (ufov_erode, cfov_erode, center_erode), int(window_size), self.threshold)
+        shape = (-(-a.shape[1] // b), -(-a.shape[2] // b))
+        return TomographicUniformityVolume(rows[0], int(window_size), shape, _DeviceArrays(cleaned, masks, mean), 0)
+
+    def analyze(self, first_frame: int = 0, last_frame: int = -1, ufov_ratio: float = 0.8, cfov_ratio: float = 0.75,
+                center_ratio: float = 0.4, threshold: float = 0.75, window_size: int = 5) -> None:
+        """Uniformity of the mean of slices `first_frame` up to (not including) `last_frame` (0-based; negative counts from the end),
+        as PlanarUniformity.analyze with `ufov_ratio`, `cfov_ratio`, `threshold` and `window_size`, and the center-to-border ratio of
+        a center FOV of `center_ratio` x `ufov_ratio`."""
+        self.threshold = threshold
+        first, last = _slab(len(self.stack.frames), first_frame, last_frame)
+        frame0 = self.stack.frames[0]
+        self.first_frame, self.last_frame = first + 1, last + 1
+        if last == 0:                       # an empty slab: an all-nan mean frame with nothing above the threshold
+            self.stack.frames = [frame0]
+            frame0.array = np.full(np.shape(frame0.array), np.nan)
+            _warn_empty_slab()
+            raise ValueError(_EMPTY_MAX)
+        if not hasattr(self, "_volume"):
+            a = self.stack._pixels
+            if a.dtype == np.uint8:
+                a = a.astype(np.uint16)
+            elif a.dtype != np.uint16:
+                raise NotImplementedError(f"nuclear frames of dtype {a.dtype.name} are not supported (uint8 or uint16)")
+            self._volume = a
+        erode = (1 - ufov_ratio, 1 - cfov_ratio * ufov_ratio, 1 - center_ratio * ufov_ratio)
+        res = self._run(first, last, *erode, window_size)
+        self.stack.frames = [_SlabMeanFrame(frame0, res._arrays)]
+        if res.status == nat.NM_NO_COMPONENT:
+            if np.isnan(res.row["threshold"]):
+                _warn_empty_threshold()
+            raise ValueError(_EMPTY_MAX)
+        self._analysed = {"first": first, "last": last, "ufov": erode[0], "cfov": erode[1], "center": center_ratio * ufov_ratio,
+                          "window": window_size, "result": res}
+        self.frame_results = {self.frame_key: {"ufov": res.ufov, "cfov": res.cfov, "binned_frame": res.binned_frame}}
+        self.center_ratio = self.center_border_ratio(center_ratio=center_ratio * ufov_ratio, window_size=window_size)
+
+    def results_data(self, as_dict: bool = False, as_json: bool = False, by_alias: bool = False, exclude: set[str] | None = None):
+        """ResultsDataMixin's results_data: the reference's class resolves it before PlanarUniformity's"""
+        return ResultsDataMixin.results_data(self, as_dict=as_dict, as_json=as_json, by_alias=by_alias, exclude=exclude)
+
+    def _generate_results_data(self) -> TomographicUniformityResults:
+        """Return the results as a structure."""
+        return TomographicUniformityResults(
+            cfov_integral_uniformity=self.frame_result["cfov"].integral_uniformity,
+            cfov_differential_uniformity=self.frame_result["cfov"].differential_uniformity,
+            ufov_integral_uniformity=self.frame_result["ufov"].integral_uniformity,
+            ufov_differential_uniformity=self.frame_result["ufov"].differential_uniformity,
+            center_border_ratio=self.center_ratio,
+            first_frame=self.first_frame,
+            last_frame=self.last_frame,
+        )
+
+    def results(self) -> str:
+        """Return a string representation of the results."""
+        return (
+            f"Tomographic Uniformity results for {self.path.name}\n"
+            f"Frames: {self.first_frame}:{self.last_frame}\n"
+            f"CFOV Integral Uniformity: {self.frame_result['cfov'].integral_uniformity:.3f}%\n"
+            f"CFOV Differential Uniformity: {self.frame_result['cfov'].differential_uniformity:.3f}%\n"
+            f"UFOV Integral Uniformity: {self.frame_result['ufov'].integral_uniformity:.3f}%\n"
+            f"UFOV Differential Uniformity: {self.frame_result['ufov'].differential_uniformity:.3f}%\n"
+            f"Center-to-Border ratio: {self.center_ratio:.3f}\n"
+        )
 
 
 # ---------------------------------------------------------------------------------------------------- TomographicContrast
