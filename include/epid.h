@@ -545,6 +545,14 @@ int32_t epid_roi_stats(epid_ctx* ctx, const epid_batch* b, int32_t nroi, const d
                        double* std, double* mn, double* mx);
 /* WeightedCentroid.calculate (metrics/image.py:959-983): cx = sum(x * a) / sum(a), cy likewise; total = sum(a) (may be NULL). */
 int32_t epid_weighted_centroid(epid_ctx* ctx, const epid_batch* b, double* cx, double* cy, double* total);
+/* DiskROI / HighContrastDiskROI statistics (core/roi.py:39-190, 411-478): for disk i, disks[i] = (frame index, centre row, centre
+ * column, radius), the pixels arr[skimage.draw.disk((cy, cx), r)] of that frame of the batch (raster order; negative indices wrap as
+ * numpy's fancy indexing does) -> count / mean / std / min / max / median [ndisk] (any may be NULL), each equal bit for bit to
+ * np.mean / np.std / np.min / np.max / np.median of those pixels.  Any dtype.  An empty disk has count 0 and NaN elsewhere; a NaN pixel
+ * makes min, max and median NaN.  A member pixel at or beyond the frame's size (numpy's IndexError) returns EPID_ERR_INVALID; a bounding
+ * box of more than 16384 rows or columns EPID_ERR_UNSUPPORTED. */
+int32_t epid_disk_stats(epid_ctx* ctx, const epid_batch* b, int32_t ndisk, const double* disks, double* count, double* mean,
+                        double* std, double* mn, double* mx, double* median);
 
 /* ----------------------------------------------------------------------------------------- VMAT (DRGS / DRMLC) and DLG
  * VMATBase.__init__ / analyze, VMATLinearBase._identify_images / _roi_profiles / _calculate_segments, Segment.r_corr / stdev,

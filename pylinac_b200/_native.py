@@ -323,6 +323,7 @@ _SIGNATURES = {
     "epid_disk_locate": [_P, _P, _P, _P],
     "epid_roi_stats": [_P, _P, C.c_int32, _P, _P, _P, _P, _P, _P],
     "epid_weighted_centroid": [_P, _P, _P, _P, _P],
+    "epid_disk_stats": [_P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P],
     "epid_vmat_analyze": [_P, _P, _P, C.POINTER(VmatParams), _P],
     "epid_divide": [_P, _P, _P, _P, C.POINTER(_P)],
     "epid_dlg_analyze": [_P, _P, C.c_int32, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P],
@@ -905,6 +906,19 @@ def roi_stats(ctx: Context, frames, verts_xy) -> dict:
         out = {k: np.empty((n, len(v))) for k in ("count", "mean", "std", "min", "max")}
         check(lib().epid_roi_stats(ctx.handle, b.handle, len(v), _ptr(v), _ptr(out["count"]), _ptr(out["mean"]), _ptr(out["std"]),
                                    _ptr(out["min"]), _ptr(out["max"])))
+    return out
+
+
+DISK_STATS = ("count", "mean", "std", "min", "max", "median")
+
+
+def disk_stats(ctx: Context, frames, disks) -> dict:
+    """DiskROI statistics of a batch: disks [ndisk, 4] rows (frame index, centre row, centre column, radius) -> dict of [ndisk]
+    float64 arrays (count, mean, std, min, max, median), each numpy's value over arr[skimage.draw.disk((cy, cx), r)] of that frame."""
+    d = np.ascontiguousarray(disks, dtype=np.float64).reshape(-1, 4)
+    out = {k: np.empty(len(d)) for k in DISK_STATS}
+    with batch_for(ctx, frames) as b:
+        check(lib().epid_disk_stats(ctx.handle, b.handle, len(d), _ptr(d), *(_ptr(out[k]) for k in DISK_STATS)))
     return out
 
 

@@ -7,14 +7,18 @@
 //                           rule is restated from its documentation / source as recalled (parity unpinned at that boundary); for
 //                           axis-aligned rectangles with integer corners it reduces to a plain slice.
 //   epid_weighted_centroid  WeightedCentroid.calculate (metrics/image.py:959-983): sum(idx * a) / sum(a) along both axes.
+//   epid_disk_stats         DiskROI / HighContrastDiskROI (core/roi.py:39-190, 411-478): np.mean / np.std / np.min / np.max /
+//                           np.median of arr[skimage.draw.disk((cy, cx), r)], bit for bit, in numpy's own summation orders.
 //
 // One CTA per (frame, ROI).  Integer dtypes accumulate exact 64-bit sums (count, sum, sum of squares, index-weighted sums); float
 // dtypes accumulate in fp64.  std = sqrt(mean(|x - mean|^2)) as numpy defines it, evaluated from the exact moments for integers.
+// epid_disk_stats runs one CTA per disk and evaluates numpy's expressions instead (see k_disk_stats).
 #include <cmath>
 #include <type_traits>
 #include <vector>
 
 #include "common.cuh"
+#include "np_sum.cuh"
 #include "roi.cuh"
 
 namespace epid {
@@ -145,6 +149,274 @@ static int do_wc(epid_ctx* ctx, const epid_batch* b, double* d_part) {
     return EPID_OK;
 }
 
+
+// ---------------------------------------------------------------------------------------------------- disk statistics
+// The pixels of skimage.draw.disk((cy, cx), r) without `shape` (ellipse with rotation 0): the bounding box ceil(c - r) .. floor(c + r),
+// float offsets (i - (cy - r0)) / r and (j - (cx - c0)) / r from the centre, membership a*a + b*b < 1 (built with -fmad=false, so it
+// rounds as numpy does), raster order; arr[rr, cc] wraps negative indices.  The member columns of one row are one run (the test is
+// monotone in |j - cx| after rounding), so each row is (first column, length) and a prefix over the lengths maps a raster index to its
+// pixel: the pairwise sums read the frame through that map and nothing is gathered.
+//
+// numpy's expressions, per dtype (numpy/_core/_methods.py _mean / _var, lib/_function_base_impl.py median):
+//   mean    integers: float64 pairwise sums over the casting buffer's chunks of 8192 values, added in sequence from 0, / n;
+//           float32: a float32 pairwise sum, float32(float64(sum) / n); float64: 0 + one pairwise sum, / n.
+//   std     d = x - mean in the mean's type, d * d, 0 + one pairwise sum of the squares (no cast, no chunks), var as the mean is
+//           formed, sqrt in that type.
+//   median  the one or two middle order statistics (radix select over order-preserving keys, 8 bits a pass), then np.mean of them;
+//           any NaN makes it NaN (numpy's _median_nancheck), as it does min and max.
+constexpr int DISK_THREADS = 256, DISK_LOG_THREADS = 8, DISK_WARPS = DISK_THREADS / 32;
+constexpr int DISK_MAX_ROWS = 16384;          // rows (and columns) of a disk's bounding box: the row table lives in shared memory
+constexpr long long NP_CAST_BUFFER = 8192;    // numpy's ufunc buffer: a cast reduction sums in chunks of this many values
+
+template <typename T> struct DiskTraits {      // unsigned integers of 8 / 16 bits
+    using Key = uint32_t; using Acc = double;
+    static constexpr bool integral = true;
+    __device__ static Key key(T v) { return v; }
+    __device__ static T value(Key k) { return (T)k; }
+};
+template <> struct DiskTraits<int16_t> {
+    using Key = uint32_t; using Acc = double;
+    static constexpr bool integral = true;
+    __device__ static Key key(int16_t v) { return (uint32_t)(uint16_t)v ^ 0x8000u; }
+    __device__ static int16_t value(Key k) { return (int16_t)(uint16_t)(k ^ 0x8000u); }
+};
+template <> struct DiskTraits<int32_t> {
+    using Key = uint32_t; using Acc = double;
+    static constexpr bool integral = true;
+    __device__ static Key key(int32_t v) { return (uint32_t)v ^ 0x80000000u; }
+    __device__ static int32_t value(Key k) { return (int32_t)(k ^ 0x80000000u); }
+};
+template <> struct DiskTraits<long long> {
+    using Key = unsigned long long; using Acc = double;
+    static constexpr bool integral = true;
+    __device__ static Key key(long long v) { return (unsigned long long)v ^ 0x8000000000000000ull; }
+    __device__ static long long value(Key k) { return (long long)(k ^ 0x8000000000000000ull); }
+};
+template <> struct DiskTraits<float> {
+    using Key = uint32_t; using Acc = float;
+    static constexpr bool integral = false;
+    __device__ static Key key(float v) { const uint32_t u = __float_as_uint(v); return (u & 0x80000000u) ? ~u : u | 0x80000000u; }
+    __device__ static float value(Key k) { return __uint_as_float((k & 0x80000000u) ? k & 0x7fffffffu : ~k); }
+};
+template <> struct DiskTraits<double> {
+    using Key = unsigned long long; using Acc = double;
+    static constexpr bool integral = false;
+    __device__ static Key key(double v) {
+        const unsigned long long u = (unsigned long long)__double_as_longlong(v);
+        return (u & 0x8000000000000000ull) ? ~u : u | 0x8000000000000000ull;
+    }
+    __device__ static double value(Key k) {
+        return __longlong_as_double((long long)((k & 0x8000000000000000ull) ? k & 0x7fffffffffffffffull : ~k));
+    }
+};
+
+struct DiskOut { double count, mean, std, mn, mx, median; };   // count < 0: a member pixel lies beyond the frame (numpy's IndexError)
+
+// skimage.draw.disk's bounding box of one disk: rows r0 .. r0 + bh - 1, columns c0 .. c0 + bw - 1 (bh, bw >= 0)
+struct DiskBox { long long r0, c0, bh, bw; };
+__host__ __device__ inline DiskBox disk_box(double cy, double cx, double R) {
+    R = fabs(R);                                     // skimage's rotated radius |r cos 0| + r sin 0
+    DiskBox b;
+    b.r0 = (long long)ceil(cy - R);
+    b.c0 = (long long)ceil(cx - R);
+    b.bh = (long long)floor(cy + R) - b.r0 + 1;
+    b.bw = (long long)floor(cx + R) - b.c0 + 1;
+    if (b.bh < 0) b.bh = 0;
+    if (b.bw < 0) b.bw = 0;
+    return b;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(DISK_THREADS)
+k_disk_stats(const T* __restrict__ data, int H, int W, const double* __restrict__ disks, DiskOut* __restrict__ out) {
+    using Tr = DiskTraits<T>;
+    using K = typename Tr::Key;
+    using A = typename Tr::Acc;
+    extern __shared__ int disk_rows[];              // lo[bh]: first member column; pre[bh + 1]: members before each row
+    __shared__ A slots[DISK_THREADS];
+    __shared__ unsigned int hist[256];
+    __shared__ long long part[DISK_THREADS];
+    __shared__ double wmn[DISK_WARPS], wmx[DISK_WARPS];
+    __shared__ int s_bad, s_nan, s_digit;
+    __shared__ long long s_k, s_eq;
+    __shared__ unsigned long long s_next;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const double* dk = disks + (size_t)blockIdx.x * 4;
+    const T* f = data + (size_t)(long long)dk[0] * H * W;
+    const double cy = dk[1], cx = dk[2], R = dk[3];
+    const DiskBox box = disk_box(cy, cx, R);
+    const int bh = (int)box.bh, bw = (int)box.bw;
+    const double sr = cy - (double)box.r0, sc = cx - (double)box.c0;   // skimage's `shifted = center - upper_left`
+    int* lo = disk_rows;
+    int* pre = disk_rows + bh;
+    if (tid == 0) { s_bad = 0; s_nan = 0; pre[0] = 0; }
+    __syncthreads();
+
+    // each row's run of member columns, and numpy's bounds check of every member index
+    for (int i = tid; i < bh; i += DISK_THREADS) {
+        const double a = ((double)i - sr) / R;
+        const double aa = a * a;
+        int first = -1, last = -2;
+        for (int j = 0; j < bw; j++) {
+            const double b = ((double)j - sc) / R;
+            if (aa + b * b < 1.0) { if (first < 0) first = j; last = j; }
+        }
+        const int len = last - first + 1;
+        lo[i] = first < 0 ? 0 : first;
+        pre[i + 1] = len;
+        if (len > 0) {
+            const long long r = box.r0 + i, c_first = box.c0 + first, c_last = box.c0 + last;
+            if (r < -H || r >= H || c_first < -W || c_last >= W) s_bad = 1;
+        }
+    }
+    __syncthreads();
+    // prefix over the run lengths: a serial chunk per thread, one serial pass over the chunk totals
+    const int chunk = (bh + DISK_THREADS - 1) / DISK_THREADS;
+    const int i0 = min(bh, tid * chunk), i1 = min(bh, i0 + chunk);
+    long long run = 0;
+    for (int i = i0; i < i1; i++) run += pre[i + 1];
+    part[tid] = run;
+    __syncthreads();
+    if (tid == 0) {
+        long long acc = 0;
+        for (int t = 0; t < DISK_THREADS; t++) { const long long v = part[t]; part[t] = acc; acc += v; }
+    }
+    __syncthreads();
+    run = part[tid];
+    for (int i = i0; i < i1; i++) { run += pre[i + 1]; pre[i + 1] = (int)run; }
+    __syncthreads();
+    const long long n = bh > 0 ? pre[bh] : 0;
+    DiskOut o;
+    o.count = (double)n;
+    o.mean = o.std = o.mn = o.mx = o.median = NAN;
+    if (s_bad || n == 0) {
+        if (s_bad) o.count = -1.0;
+        if (tid == 0) out[blockIdx.x] = o;
+        return;
+    }
+    auto pixel = [&](int i, long long j) -> T {      // member j of row i, negative indices wrapped as numpy's fancy indexing does
+        long long r = box.r0 + i, c = box.c0 + lo[i] + j;
+        if (r < 0) r += H;
+        if (c < 0) c += W;
+        return f[r * W + c];
+    };
+    auto at = [&](long long k) -> T {                // raster index k -> its pixel: the last row i with pre[i] <= k
+        int a = 0, b = bh - 1;
+        while (a < b) {
+            const int m = (a + b + 1) >> 1;
+            if (pre[m] <= k) a = m; else b = m - 1;
+        }
+        return pixel(a, k - pre[a]);
+    };
+
+    // min / max / NaN, in any order
+    double mn = INFINITY, mx = -INFINITY;
+    int has_nan = 0;
+    for (int i = warp; i < bh; i += DISK_WARPS) {
+        const int len = pre[i + 1] - pre[i];
+        for (int j = lane; j < len; j += 32) {
+            const double v = (double)pixel(i, j);
+            if (v != v) has_nan = 1;
+            mn = fmin(mn, v);
+            mx = fmax(mx, v);
+        }
+    }
+    for (int off = 16; off > 0; off >>= 1) {
+        mn = fmin(mn, __shfl_xor_sync(0xffffffffu, mn, off));
+        mx = fmax(mx, __shfl_xor_sync(0xffffffffu, mx, off));
+    }
+    if (lane == 0) { wmn[warp] = mn; wmx[warp] = mx; }
+    if (has_nan) s_nan = 1;
+    __syncthreads();
+    const bool any_nan = s_nan != 0;
+    if (!any_nan) {
+        mn = wmn[0];
+        mx = wmx[0];
+        for (int w = 1; w < DISK_WARPS; w++) { mn = fmin(mn, wmn[w]); mx = fmax(mx, wmx[w]); }
+        o.mn = mn;
+        o.mx = mx;
+    }
+
+    // np.mean
+    A sum = 0.0;
+    const long long step = Tr::integral ? NP_CAST_BUFFER : n;
+    for (long long c0 = 0; c0 < n; c0 += step) {
+        const long long len = min(step, n - c0);
+        sum = sum + np::block_pw([&](long long k) -> A { return (A)at(c0 + k); }, len, DISK_LOG_THREADS, slots);
+    }
+    const A mean = (A)((double)sum / (double)n);
+    o.mean = (double)mean;
+    // np.std
+    const A ss = (A)0.0 + np::block_pw([&](long long k) -> A { const A d = (A)at(k) - mean; return d * d; }, n, DISK_LOG_THREADS, slots);
+    const A var = (A)((double)ss / (double)n);
+    o.std = (double)sqrt(var);
+
+    // np.median: rank (n - 1) / 2 by radix select, and for even n the next order statistic
+    if (!any_nan) {
+        K prefix = 0, mask = 0;
+        long long k = n % 2 ? n / 2 : n / 2 - 1;
+        for (int shift = 8 * ((int)sizeof(T) - 1); shift >= 0; shift -= 8) {
+            for (int b = tid; b < 256; b += DISK_THREADS) hist[b] = 0;
+            __syncthreads();
+            for (int i = warp; i < bh; i += DISK_WARPS) {
+                const int len = pre[i + 1] - pre[i];
+                for (int j = lane; j < len; j += 32) {
+                    const K key = Tr::key(pixel(i, j));
+                    if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
+                }
+            }
+            __syncthreads();
+            if (tid == 0) {
+                long long acc = 0;
+                int dg = 0;
+                for (; dg < 255; dg++) {
+                    if (k < acc + (long long)hist[dg]) break;
+                    acc += hist[dg];
+                }
+                s_digit = dg;
+                s_k = k - acc;
+                s_eq = hist[dg];
+            }
+            __syncthreads();
+            prefix |= (K)s_digit << shift;
+            mask |= (K)255u << shift;
+            k = s_k;
+        }
+        const T a = Tr::value(prefix);
+        if (n % 2) {
+            o.median = (double)(A)((double)((A)0.0 + ((A)-0.0 + (A)a)) / 1.0);
+        } else {
+            T b = a;
+            if (k + 1 >= s_eq) {                     // the next order statistic is the smallest key above a's
+                if (tid == 0) s_next = ~0ull;
+                __syncthreads();
+                unsigned long long best = ~0ull;
+                for (int i = warp; i < bh; i += DISK_WARPS) {
+                    const int len = pre[i + 1] - pre[i];
+                    for (int j = lane; j < len; j += 32) {
+                        const K key = Tr::key(pixel(i, j));
+                        if (key > prefix && (unsigned long long)key < best) best = key;
+                    }
+                }
+                atomicMin(&s_next, best);
+                __syncthreads();
+                b = Tr::value((K)s_next);
+            }
+            o.median = (double)(A)((double)((A)0.0 + (((A)-0.0 + (A)a) + (A)b)) / 2.0);
+        }
+    }
+    if (tid == 0) out[blockIdx.x] = o;
+}
+
+template <typename T>
+static int do_disk(epid_ctx* ctx, const epid_batch* b, int ndisk, const double* d_disks, DiskOut* d_out, size_t smem) {
+    if (smem > 48 * 1024) EPID_SMEM_OPT_IN(ctx, k_disk_stats<T>, smem);
+    k_disk_stats<T><<<ndisk, DISK_THREADS, smem, ctx->stream>>>((const T*)b->dptr, b->h, b->w, d_disks, d_out);
+    ctx->launches++;
+    EPID_CUDA(cudaGetLastError());
+    return EPID_OK;
+}
+
 }  // namespace epid
 
 using namespace epid;
@@ -224,6 +496,48 @@ extern "C" int32_t epid_weighted_centroid(epid_ctx* ctx, const epid_batch* b, do
             cx[fi] = t[1] / t[0];
             cy[fi] = t[2] / t[0];
         }
+    }
+    return EPID_OK;
+}
+
+extern "C" int32_t epid_disk_stats(epid_ctx* ctx, const epid_batch* b, int32_t ndisk, const double* disks, double* count, double* mean,
+                                   double* std, double* mn, double* mx, double* median) {
+    EPID_REQUIRE(ctx && b && (disks || ndisk == 0) && ndisk >= 0, EPID_ERR_INVALID, "bad argument");
+    if (ndisk == 0) return EPID_OK;
+    long long max_rows = 0;
+    for (int i = 0; i < ndisk; i++) {
+        const double* d = disks + (size_t)i * 4;
+        EPID_REQUIRE(d[0] >= 0 && d[0] < b->n && d[0] == floor(d[0]), EPID_ERR_INVALID, "disk %d: frame index %g outside the batch of %d",
+                     i, d[0], b->n);
+        EPID_REQUIRE(isfinite(d[1]) && isfinite(d[2]) && isfinite(d[3]), EPID_ERR_INVALID, "disk %d: non-finite geometry", i);
+        EPID_REQUIRE(fabs(d[1]) < 1e9 && fabs(d[2]) < 1e9 && fabs(d[3]) < 1e9, EPID_ERR_UNSUPPORTED, "disk %d: geometry beyond 1e9 px", i);
+        const DiskBox bx = disk_box(d[1], d[2], d[3]);
+        EPID_REQUIRE(bx.bh <= DISK_MAX_ROWS && bx.bw <= DISK_MAX_ROWS, EPID_ERR_UNSUPPORTED,
+                     "disk %d: a %lld x %lld bounding box exceeds %d rows or columns", i, bx.bh, bx.bw, DISK_MAX_ROWS);
+        if (bx.bh > max_rows) max_rows = bx.bh;
+    }
+    EPID_CUDA(cudaSetDevice(ctx->device));
+    const size_t nd = sizeof(double) * 4 * ndisk, no = sizeof(DiskOut) * (size_t)ndisk;
+    int rc = ensure_scratch(ctx, nd + no + 512);
+    if (rc != EPID_OK) return rc;
+    double* d_disks = (double*)ctx->scratch;
+    DiskOut* d_out = (DiskOut*)((char*)ctx->scratch + (nd + 255) / 256 * 256);
+    EPID_CUDA(cudaMemcpyAsync(d_disks, disks, nd, cudaMemcpyHostToDevice, ctx->stream));
+    const size_t smem = sizeof(int) * (size_t)(2 * max_rows + 1);
+    EPID_DISPATCH_ROI(b->dtype, do_disk, ctx, b, ndisk, d_disks, d_out, smem);
+    if (rc != EPID_OK) return rc;
+    std::vector<DiskOut> h(ndisk);
+    EPID_CUDA(cudaMemcpyAsync(h.data(), d_out, no, cudaMemcpyDeviceToHost, ctx->stream));
+    EPID_CUDA(cudaStreamSynchronize(ctx->stream));
+    for (int i = 0; i < ndisk; i++) {
+        const DiskOut& o = h[i];
+        EPID_REQUIRE(o.count >= 0, EPID_ERR_INVALID, "disk %d: a member pixel lies beyond the %d x %d frame", i, b->h, b->w);
+        if (count) count[i] = o.count;
+        if (mean) mean[i] = o.mean;
+        if (std) std[i] = o.std;
+        if (mn) mn[i] = o.mn;
+        if (mx) mx[i] = o.mx;
+        if (median) median[i] = o.median;
     }
     return EPID_OK;
 }

@@ -7,7 +7,9 @@ to the reference.  The cleaned frames and FOV masks stay on the device until an 
 frame sums from epid_frame_stats.  TomographicContrast makes one device call for the slice analysis of a batch of SPECT volumes and
 one for all its sphere searches (csrc/nuclear_tomo.cu), bit-identical to the reference.  TomographicUniformity averages a slab of
 slices and runs the planar pipeline on that float64 frame, with a third (center) FOV, in one device call per batch
-(csrc/nuclear_tu.cu), bit-identical to the reference.  The other nuclear tests are not ported yet (DESIGN.md section 6).
+(csrc/nuclear_tu.cu), bit-identical to the reference.  QuadrantResolution takes the mean and standard deviation of four disk ROIs
+from one device call (epid_disk_stats, csrc/roi.cu), equal bit for bit to numpy's, and forms the moments MTF on the host in the
+reference's expressions.  The other nuclear tests are not ported yet (DESIGN.md section 6).
 """
 from __future__ import annotations
 
@@ -25,6 +27,8 @@ from pydantic import BaseModel
 from . import _native as nat
 from .core.geometry import Point, direction_to_coords
 from .core.image import NMImageStack
+from .core.mtf import MomentMTF
+from .core.roi import HighContrastDiskROI, check_disk_bounds, disk_stats_dtype, fill_disk_stats
 from .core.utilities import ResultBase, ResultsDataMixin
 from .core.warnings import capture_warnings
 
@@ -963,3 +967,117 @@ class TomographicContrast(ResultsDataMixin[TomographicContrastResults]):
                                            mean_contrast=roi.mean_contrast, max_contrast=roi.max_contrast)
                      for idx, roi in self.rois.items()},
         )
+
+
+# ---------------------------------------------------------------------------------------------------- QuadrantResolution
+_QUADRANT_ANGLES = (45, -45, -135, 135)
+
+
+def _four_bar_widths(bar_widths: Sequence[float]) -> np.ndarray:
+    """the line pairs per mm of the four bar widths; any other number raises the reference's ValueError"""
+    if len(bar_widths) != 4:
+        raise ValueError("Must have 4 bar widths")
+    return 1 / (2 * np.asarray(bar_widths))
+
+
+def _quadrant_centers(rows: int, columns: int, bar_widths: Sequence[float], distance_from_center_mm: float) -> dict:
+    """{bar width: ROI centre} in the reference's order and expressions: the phantom centre is Point(Rows / 2, Columns / 2), so the
+    rows give x; a repeated bar width keeps its first position and its last centre.  Distances are used as pixels."""
+    img_center = Point(rows / 2, columns / 2)
+    centers = {}
+    for angle, spacing in zip(_QUADRANT_ANGLES, bar_widths):
+        centers[spacing] = HighContrastDiskROI._get_shifted_center(angle, distance_from_center_mm, img_center)
+    return centers
+
+
+class QuadrantResolutionFrame:
+    """The analysis of one frame of analyze_quadrant_resolution_batch: the ROIs' statistics (lists in ROI order: ``counts``,
+    ``means``, ``stds``, ``medians``, ``mins``, ``maxs``), their ``centers`` and ``bar_widths``, and the reference's ``mtf`` and
+    ``quadrants``, which raise the reference's exceptions.  An empty ROI has a NaN mean, std and median, without numpy's warnings."""
+
+    def __init__(self, lpmm: np.ndarray, centers: dict, stats: dict):
+        self.lpmm, self.bar_widths, self.centers = lpmm, list(centers), list(centers.values())
+        self.counts, self.means, self.stds = stats["count"], stats["mean"], stats["std"]
+        self.medians, self.mins, self.maxs = stats["median"], stats["min"], stats["max"]
+
+    @cached_property
+    def mtf(self) -> MomentMTF:
+        return MomentMTF(self.lpmm, self.means, self.stds)
+
+    @property
+    def quadrants(self) -> dict[str, dict[str, float]]:
+        """QuadrantResolutionResults.quadrants"""
+        return _quadrants(self.mtf)
+
+
+def analyze_quadrant_resolution_batch(frames, bar_widths: Sequence[float], roi_diameter_mm: float = 70,
+                                      distance_from_center_mm: float = 130, *, device: int | None = None) -> list[QuadrantResolutionFrame]:
+    """``QuadrantResolution.analyze(bar_widths, roi_diameter_mm, distance_from_center_mm)`` for every frame of `frames` (an [n, h, w]
+    or [h, w] ndarray or a device Batch, any dtype the disk statistics read), with the statistics of all its disks from one device
+    call.  Each frame is analysed as QuadrantResolution analyses frame 0 of an h x w file.  The bar-width count and a disk beyond the
+    frame raise the reference's ValueError and IndexError before any device call."""
+    lpmm = _four_bar_widths(bar_widths)
+    if isinstance(frames, nat.Batch):
+        (n, h, w), _ = frames.shape_dtype
+    else:
+        frames = np.asarray(frames)
+        frames = frames[None] if frames.ndim == 2 else frames
+        if frames.ndim != 3:
+            raise ValueError(f"frames must be [n, h, w] or [h, w], got {frames.ndim}-D")
+        frames = disk_stats_dtype(frames)
+        n, h, w = frames.shape
+    centers = _quadrant_centers(h, w, bar_widths, distance_from_center_mm)
+    for c in centers.values():
+        check_disk_bounds((h, w), c.y, c.x, roi_diameter_mm)
+    disks = [(f, c.y, c.x, roi_diameter_mm) for f in range(n) for c in centers.values()]
+    out = nat.disk_stats(nat.Context.default(device), frames, disks)
+    k = len(centers)
+    return [QuadrantResolutionFrame(lpmm, centers, {name: [float(v) for v in a[f * k:(f + 1) * k]] for name, a in out.items()})
+            for f in range(n)]
+
+
+def _quadrants(mtf: MomentMTF) -> dict[str, dict[str, float]]:
+    return {
+        f"{idx + 1}": {"mtf": m, "fwhm": fwhm, "lpmm": lpmm, "spacing": 1 / (lpmm * 2)}
+        for idx, ((lpmm, m), fwhm) in enumerate(zip(mtf.mtfs.items(), mtf.fwhms.values()))
+    }
+
+
+class QuadrantResolutionResults(ResultBase):
+    quadrants: dict[str, dict[str, float]]  #: quadrant idx: {'mtf': mtf, 'fwhm': fwhm, 'lpmm': lpmm, 'spacing': bar width}
+
+
+@capture_warnings
+class QuadrantResolution(ResultsDataMixin[QuadrantResolutionResults]):
+    """MTF and FWHM of a 4-quadrant bar phantom image (nuclear.py:1248-1367): the moments MTF of Hander et al. of one disk ROI per
+    quadrant of frame 0."""
+
+    rois: dict[float, HighContrastDiskROI]
+    mtf: MomentMTF
+
+    def __init__(self, path: str | Path) -> None:
+        super().__init__()
+        self.stack = NMImageStack(path)
+        self.path = Path(path)
+
+    def analyze(self, bar_widths: Sequence[float], roi_diameter_mm: float = 70, distance_from_center_mm: float = 130) -> None:
+        """The MTF and FWHM of each quadrant, from disk ROIs of `roi_diameter_mm` (used as a radius in pixels) whose centres lie
+        `distance_from_center_mm` (pixels) from the image centre.  `bar_widths`: the four bar widths in mm."""
+        lpmm = _four_bar_widths(bar_widths)
+        centers = _quadrant_centers(self.stack.metadata.Rows, self.stack.metadata.Columns, bar_widths, distance_from_center_mm)
+        self.rois = {spacing: HighContrastDiskROI(self.stack.frames[0], radius=roi_diameter_mm, center=c, contrast_threshold=0)
+                     for spacing, c in centers.items()}
+        fill_disk_stats(list(self.rois.values()))
+        self.mtf = MomentMTF.from_high_contrast_diskset(lpmm, list(self.rois.values()))
+
+    def results(self) -> str:
+        """Return a string representation of the results."""
+        s = f"Quadrant Resolution results for {self.path.name}\n"
+        for quadrant, ((lpmm, mtf), fwhm) in enumerate(zip(self.mtf.mtfs.items(), self.mtf.fwhms.values())):
+            spacing = 1 / (lpmm * 2)
+            s += f"Quadrant {quadrant + 1}; Bar width: {spacing:.2f}mm; FWHM: {fwhm:.3f}mm; MTF: {mtf:.3f}\n"
+        return s
+
+    def _generate_results_data(self) -> QuadrantResolutionResults:
+        """Return the results as a structure."""
+        return QuadrantResolutionResults(quadrants=_quadrants(self.mtf))
