@@ -553,6 +553,13 @@ int32_t epid_weighted_centroid(epid_ctx* ctx, const epid_batch* b, double* cx, d
  * box of more than 16384 rows or columns EPID_ERR_UNSUPPORTED. */
 int32_t epid_disk_stats(epid_ctx* ctx, const epid_batch* b, int32_t ndisk, const double* disks, double* count, double* mean,
                         double* std, double* mn, double* mx, double* median);
+/* LowContrastDiskROI.percentile (core/roi.py:406-408): out[i * nq + k] = np.percentile(arr[skimage.draw.disk((cy, cx), r)], q_percent[k])
+ * (method "linear") of disk i, disks as for epid_disk_stats, equal bit for bit to numpy's for q_percent[k] passed as a Python number:
+ * the value of a float32 batch is numpy's float32 result, widened.  1 <= nq <= 16.  A disk with a NaN pixel, or an empty disk, gives
+ * NaN (numpy raises IndexError for an empty one).  A q_percent outside [0, 100] (checked as numpy does, in float32 for a float32 batch)
+ * returns EPID_ERR_INVALID with numpy's message; a member pixel beyond the frame returns EPID_ERR_INVALID. */
+int32_t epid_disk_percentiles(epid_ctx* ctx, const epid_batch* b, int32_t ndisk, const double* disks, int32_t nq, const double* q_percent,
+                              double* out);
 
 /* ----------------------------------------------------------------------------------------- VMAT (DRGS / DRMLC) and DLG
  * VMATBase.__init__ / analyze, VMATLinearBase._identify_images / _roi_profiles / _calculate_segments, Segment.r_corr / stdev,

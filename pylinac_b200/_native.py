@@ -324,6 +324,7 @@ _SIGNATURES = {
     "epid_roi_stats": [_P, _P, C.c_int32, _P, _P, _P, _P, _P, _P],
     "epid_weighted_centroid": [_P, _P, _P, _P, _P],
     "epid_disk_stats": [_P, _P, C.c_int32, _P, _P, _P, _P, _P, _P, _P],
+    "epid_disk_percentiles": [_P, _P, C.c_int32, _P, C.c_int32, _P, _P],
     "epid_vmat_analyze": [_P, _P, _P, C.POINTER(VmatParams), _P],
     "epid_divide": [_P, _P, _P, _P, C.POINTER(_P)],
     "epid_dlg_analyze": [_P, _P, C.c_int32, _P, _P, C.c_int32, C.c_int32, _P, _P, _P, _P, _P],
@@ -919,6 +920,17 @@ def disk_stats(ctx: Context, frames, disks) -> dict:
     out = {k: np.empty(len(d)) for k in DISK_STATS}
     with batch_for(ctx, frames) as b:
         check(lib().epid_disk_stats(ctx.handle, b.handle, len(d), _ptr(d), *(_ptr(out[k]) for k in DISK_STATS)))
+    return out
+
+
+def disk_percentiles(ctx: Context, frames, disks, q) -> np.ndarray:
+    """np.percentile(arr[skimage.draw.disk((cy, cx), r)], q) of each disk of `disks` (rows as for disk_stats) for each q of `q` (1 to 16
+    Python numbers) -> float64 [ndisk, nq].  A float32 batch gives numpy's float32 values.  NaN for a disk with a NaN pixel or no pixel."""
+    d = np.ascontiguousarray(disks, dtype=np.float64).reshape(-1, 4)
+    qs = np.ascontiguousarray(q, dtype=np.float64).reshape(-1)
+    out = np.empty((len(d), len(qs)))
+    with batch_for(ctx, frames) as b:
+        check(lib().epid_disk_percentiles(ctx.handle, b.handle, len(d), _ptr(d), len(qs), _ptr(qs), _ptr(out)))
     return out
 
 

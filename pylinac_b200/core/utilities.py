@@ -20,6 +20,14 @@ def convert_to_enum(value, enum: type[Enum]) -> Enum:
     return enum(value)
 
 
+class OptionListMixin:
+    """core/utilities.py:35-45: ``options()`` lists the values of an enum-like class's public, non-callable attributes."""
+
+    @classmethod
+    def options(cls) -> list[str]:
+        return [v for k, v in cls.__dict__.items() if not k.startswith("__") and not callable(v)]
+
+
 class ResultBase(BaseModel):
     """core/utilities.py:48-66"""
 

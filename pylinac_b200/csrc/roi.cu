@@ -20,6 +20,7 @@
 #include "common.cuh"
 #include "np_sum.cuh"
 #include "roi.cuh"
+#include "stats.cuh"
 
 namespace epid {
 
@@ -226,30 +227,29 @@ __host__ __device__ inline DiskBox disk_box(double cy, double cx, double R) {
     return b;
 }
 
-template <typename T>
-__global__ void __launch_bounds__(DISK_THREADS)
-k_disk_stats(const T* __restrict__ data, int H, int W, const double* __restrict__ disks, DiskOut* __restrict__ out) {
-    using Tr = DiskTraits<T>;
-    using K = typename Tr::Key;
-    using A = typename Tr::Acc;
-    extern __shared__ int disk_rows[];              // lo[bh]: first member column; pre[bh + 1]: members before each row
-    __shared__ A slots[DISK_THREADS];
-    __shared__ unsigned int hist[256];
+// member j of row i of a disk's row table, negative indices wrapped as numpy's fancy indexing does
+template <typename T> struct DiskPixel {
+    const T* f;
+    const int* lo;
+    long long r0, c0;
+    int H, W;
+    __device__ T operator()(int i, long long j) const {
+        long long r = r0 + i, c = c0 + lo[i] + j;
+        if (r < 0) r += H;
+        if (c < 0) c += W;
+        return f[r * W + c];
+    }
+};
+
+// The row table of one disk in shared memory: lo[i] is row i's first member column and pre[i] the members before row i (pre[bh] = n),
+// with numpy's bounds check of every member index.  Returns n, or -1 when a member lies beyond the frame (numpy's IndexError).  Every
+// thread of the CTA calls it, once per CTA; kept out of line, which keeps k_disk_percentiles from spilling.
+__device__ __noinline__ long long disk_rows_table(const DiskBox& box, double sr, double sc, double R, int H, int W, int* lo, int* pre) {
     __shared__ long long part[DISK_THREADS];
-    __shared__ double wmn[DISK_WARPS], wmx[DISK_WARPS];
-    __shared__ int s_bad, s_nan, s_digit;
-    __shared__ long long s_k, s_eq;
-    __shared__ unsigned long long s_next;
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const double* dk = disks + (size_t)blockIdx.x * 4;
-    const T* f = data + (size_t)(long long)dk[0] * H * W;
-    const double cy = dk[1], cx = dk[2], R = dk[3];
-    const DiskBox box = disk_box(cy, cx, R);
+    __shared__ int s_bad;
+    const int tid = threadIdx.x;
     const int bh = (int)box.bh, bw = (int)box.bw;
-    const double sr = cy - (double)box.r0, sc = cx - (double)box.c0;   // skimage's `shifted = center - upper_left`
-    int* lo = disk_rows;
-    int* pre = disk_rows + bh;
-    if (tid == 0) { s_bad = 0; s_nan = 0; pre[0] = 0; }
+    if (tid == 0) { s_bad = 0; pre[0] = 0; }
     __syncthreads();
 
     // each row's run of member columns, and numpy's bounds check of every member index
@@ -285,21 +285,101 @@ k_disk_stats(const T* __restrict__ data, int H, int W, const double* __restrict_
     run = part[tid];
     for (int i = i0; i < i1; i++) { run += pre[i + 1]; pre[i + 1] = (int)run; }
     __syncthreads();
-    const long long n = bh > 0 ? pre[bh] : 0;
+    if (s_bad) return -1;
+    return bh > 0 ? pre[bh] : 0;
+}
+
+// The order statistics of ranks k and, with `next`, k + 1 (0-based) of the disk's pixels in DiskTraits' key order, by radix select:
+// 8 bits a pass, each pass a 256-bin shared histogram of the keys that match the digits chosen so far, so no pixel is buffered.  Rank
+// k + 1 is rank k's key again while that key's count covers it, else the smallest key above it (one more pass).  Every thread of
+// the CTA calls it with the same arguments and receives both values (b = a without `next`).
+template <typename T>
+__device__ __forceinline__ void disk_select(const DiskPixel<T>& pixel, const int* pre, int bh, long long k, bool next, T& a, T& b) {
+    using Tr = DiskTraits<T>;
+    using K = typename Tr::Key;
+    __shared__ unsigned int hist[256];
+    __shared__ int s_digit;
+    __shared__ long long s_k, s_eq;
+    __shared__ unsigned long long s_next;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    K prefix = 0, mask = 0;
+    for (int shift = 8 * ((int)sizeof(T) - 1); shift >= 0; shift -= 8) {
+        for (int d = tid; d < 256; d += DISK_THREADS) hist[d] = 0;
+        __syncthreads();
+        for (int i = warp; i < bh; i += DISK_WARPS) {
+            const int len = pre[i + 1] - pre[i];
+            for (int j = lane; j < len; j += 32) {
+                const K key = Tr::key(pixel(i, j));
+                if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
+            }
+        }
+        __syncthreads();
+        if (tid == 0) {
+            long long acc = 0;
+            int dg = 0;
+            for (; dg < 255; dg++) {
+                if (k < acc + (long long)hist[dg]) break;
+                acc += hist[dg];
+            }
+            s_digit = dg;
+            s_k = k - acc;
+            s_eq = hist[dg];
+        }
+        __syncthreads();
+        prefix |= (K)s_digit << shift;
+        mask |= (K)255u << shift;
+        k = s_k;
+    }
+    a = b = Tr::value(prefix);
+    if (next && k + 1 >= s_eq) {                     // the next order statistic is the smallest key above a's
+        if (tid == 0) s_next = ~0ull;
+        __syncthreads();
+        unsigned long long best = ~0ull;
+        for (int i = warp; i < bh; i += DISK_WARPS) {
+            const int len = pre[i + 1] - pre[i];
+            for (int j = lane; j < len; j += 32) {
+                const K key = Tr::key(pixel(i, j));
+                if (key > prefix && (unsigned long long)key < best) best = key;
+            }
+        }
+        atomicMin(&s_next, best);
+        __syncthreads();
+        b = Tr::value((K)s_next);
+    }
+}
+
+// CTAs an SM that k_disk_stats asks of ptxas: the occupancy of the kernel before its select moved into disk_select, 3 for float64 and
+// uint8 (at most 85 registers), 4 for the others (64).  The kernel is latency-bound; without a bound ptxas takes 80 to 96 registers,
+// and at 80 (3 CTAs) uint16 measured 7 % slower than at 64.  At 64 the 16- to 64-bit integers reload 80 spilled bytes.
+template <typename T> constexpr int DISK_STATS_MIN_CTAS = std::is_same<T, double>::value || std::is_same<T, uint8_t>::value ? 3 : 4;
+
+template <typename T>
+__global__ void __launch_bounds__(DISK_THREADS, DISK_STATS_MIN_CTAS<T>)
+k_disk_stats(const T* __restrict__ data, int H, int W, const double* __restrict__ disks, DiskOut* __restrict__ out) {
+    using Tr = DiskTraits<T>;
+    using A = typename Tr::Acc;
+    extern __shared__ int disk_rows[];              // lo[bh]: first member column; pre[bh + 1]: members before each row
+    __shared__ A slots[DISK_THREADS];
+    __shared__ double wmn[DISK_WARPS], wmx[DISK_WARPS];
+    __shared__ int s_nan;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const double* dk = disks + (size_t)blockIdx.x * 4;
+    const T* f = data + (size_t)(long long)dk[0] * H * W;
+    const double cy = dk[1], cx = dk[2], R = dk[3];
+    const DiskBox box = disk_box(cy, cx, R);
+    const int bh = (int)box.bh;
+    int* lo = disk_rows;
+    int* pre = disk_rows + bh;
+    if (tid == 0) s_nan = 0;
+    const long long n = disk_rows_table(box, cy - (double)box.r0, cx - (double)box.c0, R, H, W, lo, pre);   // skimage's `shifted`
     DiskOut o;
     o.count = (double)n;
     o.mean = o.std = o.mn = o.mx = o.median = NAN;
-    if (s_bad || n == 0) {
-        if (s_bad) o.count = -1.0;
+    if (n <= 0) {
         if (tid == 0) out[blockIdx.x] = o;
         return;
     }
-    auto pixel = [&](int i, long long j) -> T {      // member j of row i, negative indices wrapped as numpy's fancy indexing does
-        long long r = box.r0 + i, c = box.c0 + lo[i] + j;
-        if (r < 0) r += H;
-        if (c < 0) c += W;
-        return f[r * W + c];
-    };
+    const DiskPixel<T> pixel{f, lo, box.r0, box.c0, H, W};
     auto at = [&](long long k) -> T {                // raster index k -> its pixel: the last row i with pre[i] <= k
         int a = 0, b = bh - 1;
         while (a < b) {
@@ -351,67 +431,121 @@ k_disk_stats(const T* __restrict__ data, int H, int W, const double* __restrict_
     const A var = (A)((double)ss / (double)n);
     o.std = (double)sqrt(var);
 
-    // np.median: rank (n - 1) / 2 by radix select, and for even n the next order statistic
+    // np.median: rank (n - 1) / 2, and for even n the next order statistic
     if (!any_nan) {
-        K prefix = 0, mask = 0;
-        long long k = n % 2 ? n / 2 : n / 2 - 1;
-        for (int shift = 8 * ((int)sizeof(T) - 1); shift >= 0; shift -= 8) {
-            for (int b = tid; b < 256; b += DISK_THREADS) hist[b] = 0;
-            __syncthreads();
-            for (int i = warp; i < bh; i += DISK_WARPS) {
-                const int len = pre[i + 1] - pre[i];
-                for (int j = lane; j < len; j += 32) {
-                    const K key = Tr::key(pixel(i, j));
-                    if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
-                }
-            }
-            __syncthreads();
-            if (tid == 0) {
-                long long acc = 0;
-                int dg = 0;
-                for (; dg < 255; dg++) {
-                    if (k < acc + (long long)hist[dg]) break;
-                    acc += hist[dg];
-                }
-                s_digit = dg;
-                s_k = k - acc;
-                s_eq = hist[dg];
-            }
-            __syncthreads();
-            prefix |= (K)s_digit << shift;
-            mask |= (K)255u << shift;
-            k = s_k;
-        }
-        const T a = Tr::value(prefix);
-        if (n % 2) {
-            o.median = (double)(A)((double)((A)0.0 + ((A)-0.0 + (A)a)) / 1.0);
-        } else {
-            T b = a;
-            if (k + 1 >= s_eq) {                     // the next order statistic is the smallest key above a's
-                if (tid == 0) s_next = ~0ull;
-                __syncthreads();
-                unsigned long long best = ~0ull;
-                for (int i = warp; i < bh; i += DISK_WARPS) {
-                    const int len = pre[i + 1] - pre[i];
-                    for (int j = lane; j < len; j += 32) {
-                        const K key = Tr::key(pixel(i, j));
-                        if (key > prefix && (unsigned long long)key < best) best = key;
-                    }
-                }
-                atomicMin(&s_next, best);
-                __syncthreads();
-                b = Tr::value((K)s_next);
-            }
-            o.median = (double)(A)((double)((A)0.0 + (((A)-0.0 + (A)a) + (A)b)) / 2.0);
-        }
+        T a, b;
+        disk_select<T>(pixel, pre, bh, n % 2 ? n / 2 : n / 2 - 1, n % 2 == 0, a, b);
+        if (n % 2) o.median = (double)(A)((double)((A)0.0 + ((A)-0.0 + (A)a)) / 1.0);
+        else o.median = (double)(A)((double)((A)0.0 + (((A)-0.0 + (A)a) + (A)b)) / 2.0);
     }
     if (tid == 0) out[blockIdx.x] = o;
+}
+
+// np.percentile(arr[disk], q) (method "linear") of one disk per CTA for nq percentiles.  numpy plans and interpolates in the result's
+// type: float32 for a float32 array (q / float32(100), the virtual index and the lerp all in float32), float64 for every other dtype.
+// An integer array forms b - a in its own type, wrapping, before the lerp.  Each distinct rank the plans name is selected once, and a
+// rank k followed by k + 1 in one select.  Any NaN pixel gives NaN (np.percentile returns the NaN that sorts last).
+constexpr int DISK_MAX_Q = 16;
+template <typename T> using PctType = typename std::conditional<std::is_same<T, float>::value, float, double>::type;
+
+template <typename T>
+__global__ void __launch_bounds__(DISK_THREADS)
+k_disk_percentiles(const T* __restrict__ data, int H, int W, const double* __restrict__ disks, int nq, const double* __restrict__ q_percent,
+                   double* __restrict__ out, long long* __restrict__ count) {
+    using F = PctType<T>;
+    extern __shared__ int disk_rows[];
+    __shared__ long long s_rank[2 * DISK_MAX_Q];    // the distinct ranks the plans read, ascending
+    __shared__ T s_val[2 * DISK_MAX_Q];
+    __shared__ int s_nr, s_ia[DISK_MAX_Q], s_ib[DISK_MAX_Q];   // each q's two ranks, as indices into s_rank
+    __shared__ F s_t[DISK_MAX_Q];                   // and its weight
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const double* dk = disks + (size_t)blockIdx.x * 4;
+    const T* f = data + (size_t)(long long)dk[0] * H * W;
+    const double cy = dk[1], cx = dk[2], R = dk[3];
+    const DiskBox box = disk_box(cy, cx, R);
+    const int bh = (int)box.bh;
+    int* lo = disk_rows;
+    int* pre = disk_rows + bh;
+    const long long n = disk_rows_table(box, cy - (double)box.r0, cx - (double)box.c0, R, H, W, lo, pre);
+    if (tid == 0) count[blockIdx.x] = n;
+    double* o = out + (size_t)blockIdx.x * nq;
+    const DiskPixel<T> pixel{f, lo, box.r0, box.c0, H, W};
+    bool nan = n <= 0;
+    if constexpr (!std::is_integral<T>::value) {
+        if (!nan) for (int i = warp; i < bh; i += DISK_WARPS) {
+            const int len = pre[i + 1] - pre[i];
+            for (int j = lane; j < len; j += 32) { const T v = pixel(i, j); if (v != v) nan = true; }
+        }
+    }
+    if (__syncthreads_or(nan)) {
+        for (int k = tid; k < nq; k += DISK_THREADS) o[k] = NAN;
+        return;
+    }
+    if (tid == 0) {
+        int nr = 0;
+        for (int k = 0; k < nq; k++) {
+            const F q = (F)q_percent[k];
+            const PctPlanOf<F> p = pct_plan((int)n, q);
+            for (int u = 0; u < 2; u++) {               // insert prev, then next, into the ascending list of distinct ranks
+                const long long r = u ? p.next : p.prev;
+                int at = nr;
+                while (at > 0 && s_rank[at - 1] > r) at--;
+                if (at > 0 && s_rank[at - 1] == r) continue;
+                for (int m = nr; m > at; m--) s_rank[m] = s_rank[m - 1];
+                s_rank[at] = r;
+                nr++;
+            }
+            // numpy's weight is the virtual index less the previous index, which is -1 past the end (_get_indexes, _get_gamma); it
+            // differs from pct_plan's gamma only there and at q = -0, where it changes the sign of a zero result
+            const F vi = (F)(n - 1) * (q / (F)100.0);
+            s_t[k] = (F)((double)vi - (vi >= (F)(n - 1) ? -1.0 : (double)p.prev));
+            s_ia[k] = p.prev;                           // a rank for now; an index into s_rank below
+            s_ib[k] = p.next;
+        }
+        for (int k = 0; k < nq; k++) {
+            int ia = 0, ib = 0;
+            while (s_rank[ia] != s_ia[k]) ia++;
+            while (s_rank[ib] != s_ib[k]) ib++;
+            s_ia[k] = ia;
+            s_ib[k] = ib;
+        }
+        s_nr = nr;
+    }
+    __syncthreads();
+    for (int r = 0; r < s_nr;) {
+        const bool next = r + 1 < s_nr && s_rank[r + 1] == s_rank[r] + 1;
+        T a, b;
+        disk_select<T>(pixel, pre, bh, s_rank[r], next, a, b);
+        if (tid == 0) { s_val[r] = a; s_val[r + next] = b; }
+        r += next ? 2 : 1;
+    }
+    __syncthreads();
+    for (int k = tid; k < nq; k += DISK_THREADS) {
+        const T a = s_val[s_ia[k]], b = s_val[s_ib[k]];
+        const F t = s_t[k];
+        F d = (F)b - (F)a;
+        if constexpr (std::is_integral<T>::value) {
+            using U = typename std::make_unsigned<T>::type;
+            d = (F)(T)(U)((U)b - (U)a);
+        }
+        o[k] = (double)np_lerp_d((F)a, (F)b, d, t);
+    }
 }
 
 template <typename T>
 static int do_disk(epid_ctx* ctx, const epid_batch* b, int ndisk, const double* d_disks, DiskOut* d_out, size_t smem) {
     if (smem > 48 * 1024) EPID_SMEM_OPT_IN(ctx, k_disk_stats<T>, smem);
     k_disk_stats<T><<<ndisk, DISK_THREADS, smem, ctx->stream>>>((const T*)b->dptr, b->h, b->w, d_disks, d_out);
+    ctx->launches++;
+    EPID_CUDA(cudaGetLastError());
+    return EPID_OK;
+}
+
+template <typename T>
+static int do_disk_pct(epid_ctx* ctx, const epid_batch* b, int ndisk, const double* d_disks, int nq, const double* d_q, double* d_out,
+                       long long* d_count, size_t smem) {
+    if (smem > 48 * 1024) EPID_SMEM_OPT_IN(ctx, k_disk_percentiles<T>, smem);
+    k_disk_percentiles<T><<<ndisk, DISK_THREADS, smem, ctx->stream>>>((const T*)b->dptr, b->h, b->w, d_disks, nq, d_q, d_out, d_count);
     ctx->launches++;
     EPID_CUDA(cudaGetLastError());
     return EPID_OK;
@@ -500,11 +634,9 @@ extern "C" int32_t epid_weighted_centroid(epid_ctx* ctx, const epid_batch* b, do
     return EPID_OK;
 }
 
-extern "C" int32_t epid_disk_stats(epid_ctx* ctx, const epid_batch* b, int32_t ndisk, const double* disks, double* count, double* mean,
-                                   double* std, double* mn, double* mx, double* median) {
-    EPID_REQUIRE(ctx && b && (disks || ndisk == 0) && ndisk >= 0, EPID_ERR_INVALID, "bad argument");
-    if (ndisk == 0) return EPID_OK;
-    long long max_rows = 0;
+// the disk rows' checks shared by the disk entry points; *max_rows: the most bounding-box rows of any disk
+static int check_disks(const epid_batch* b, int ndisk, const double* disks, long long* max_rows) {
+    *max_rows = 0;
     for (int i = 0; i < ndisk; i++) {
         const double* d = disks + (size_t)i * 4;
         EPID_REQUIRE(d[0] >= 0 && d[0] < b->n && d[0] == floor(d[0]), EPID_ERR_INVALID, "disk %d: frame index %g outside the batch of %d",
@@ -514,11 +646,21 @@ extern "C" int32_t epid_disk_stats(epid_ctx* ctx, const epid_batch* b, int32_t n
         const DiskBox bx = disk_box(d[1], d[2], d[3]);
         EPID_REQUIRE(bx.bh <= DISK_MAX_ROWS && bx.bw <= DISK_MAX_ROWS, EPID_ERR_UNSUPPORTED,
                      "disk %d: a %lld x %lld bounding box exceeds %d rows or columns", i, bx.bh, bx.bw, DISK_MAX_ROWS);
-        if (bx.bh > max_rows) max_rows = bx.bh;
+        if (bx.bh > *max_rows) *max_rows = bx.bh;
     }
+    return EPID_OK;
+}
+
+extern "C" int32_t epid_disk_stats(epid_ctx* ctx, const epid_batch* b, int32_t ndisk, const double* disks, double* count, double* mean,
+                                   double* std, double* mn, double* mx, double* median) {
+    EPID_REQUIRE(ctx && b && (disks || ndisk == 0) && ndisk >= 0, EPID_ERR_INVALID, "bad argument");
+    if (ndisk == 0) return EPID_OK;
+    long long max_rows = 0;
+    int rc = check_disks(b, ndisk, disks, &max_rows);
+    if (rc != EPID_OK) return rc;
     EPID_CUDA(cudaSetDevice(ctx->device));
     const size_t nd = sizeof(double) * 4 * ndisk, no = sizeof(DiskOut) * (size_t)ndisk;
-    int rc = ensure_scratch(ctx, nd + no + 512);
+    rc = ensure_scratch(ctx, nd + no + 512);
     if (rc != EPID_OK) return rc;
     double* d_disks = (double*)ctx->scratch;
     DiskOut* d_out = (DiskOut*)((char*)ctx->scratch + (nd + 255) / 256 * 256);
@@ -539,5 +681,42 @@ extern "C" int32_t epid_disk_stats(epid_ctx* ctx, const epid_batch* b, int32_t n
         if (mx) mx[i] = o.mx;
         if (median) median[i] = o.median;
     }
+    return EPID_OK;
+}
+
+extern "C" int32_t epid_disk_percentiles(epid_ctx* ctx, const epid_batch* b, int32_t ndisk, const double* disks, int32_t nq,
+                                         const double* q_percent, double* out) {
+    EPID_REQUIRE(ctx && b && (disks || ndisk == 0) && ndisk >= 0, EPID_ERR_INVALID, "bad argument");
+    EPID_REQUIRE(nq >= 1 && nq <= DISK_MAX_Q && q_percent && (out || ndisk == 0), EPID_ERR_INVALID, "%d percentiles: 1 to %d are supported",
+                 nq, DISK_MAX_Q);
+    for (int k = 0; k < nq; k++) {             // np.percentile checks q / 100 in the type it plans in (float32 for a float32 batch)
+        const double q = b->dtype == EPID_F32 ? (double)((float)q_percent[k] / 100.0f) : q_percent[k] / 100.0;
+        EPID_REQUIRE(q >= 0.0 && q <= 1.0, EPID_ERR_INVALID, "Percentiles must be in the range [0, 100]");
+    }
+    if (ndisk == 0) return EPID_OK;
+    long long max_rows = 0;
+    int rc = check_disks(b, ndisk, disks, &max_rows);
+    if (rc != EPID_OK) return rc;
+    EPID_CUDA(cudaSetDevice(ctx->device));
+    const size_t nd = sizeof(double) * 4 * ndisk, nqb = sizeof(double) * nq, no = sizeof(double) * (size_t)ndisk * nq,
+                 nc = sizeof(long long) * (size_t)ndisk;
+    auto up = [](size_t v) { return (v + 255) / 256 * 256; };
+    rc = ensure_scratch(ctx, up(nd) + up(nqb) + up(no) + nc + 256);
+    if (rc != EPID_OK) return rc;
+    double* d_disks = (double*)ctx->scratch;
+    double* d_q = (double*)((char*)d_disks + up(nd));
+    double* d_out = (double*)((char*)d_q + up(nqb));
+    long long* d_count = (long long*)((char*)d_out + up(no));
+    EPID_CUDA(cudaMemcpyAsync(d_disks, disks, nd, cudaMemcpyHostToDevice, ctx->stream));
+    EPID_CUDA(cudaMemcpyAsync(d_q, q_percent, nqb, cudaMemcpyHostToDevice, ctx->stream));
+    const size_t smem = sizeof(int) * (size_t)(2 * max_rows + 1);
+    EPID_DISPATCH_ROI(b->dtype, do_disk_pct, ctx, b, ndisk, d_disks, nq, d_q, d_out, d_count, smem);
+    if (rc != EPID_OK) return rc;
+    std::vector<long long> cnt(ndisk);
+    EPID_CUDA(cudaMemcpyAsync(out, d_out, no, cudaMemcpyDeviceToHost, ctx->stream));
+    EPID_CUDA(cudaMemcpyAsync(cnt.data(), d_count, nc, cudaMemcpyDeviceToHost, ctx->stream));
+    EPID_CUDA(cudaStreamSynchronize(ctx->stream));
+    for (int i = 0; i < ndisk; i++)
+        EPID_REQUIRE(cnt[i] >= 0, EPID_ERR_INVALID, "disk %d: a member pixel lies beyond the %d x %d frame", i, b->h, b->w);
     return EPID_OK;
 }

@@ -43,20 +43,23 @@ struct FrameStats {  // per frame, device memory
 
 // np.percentile(a, q_percent) with method="linear" over n values reads the sorted values at ranks prev and next and interpolates with
 // gamma.  numpy's virtual index for "linear" is (n - 1) * q with q = q_percent / 100; written any other way it rounds differently for
-// some (n, q) and the percentile moves by many ulps.  An index at or past n - 1 takes the last value, one below 0 the first.
-struct PctPlan { int prev, next; double gamma; };
+// some (n, q) and the percentile moves by many ulps.  An index at or past n - 1 takes the last value, one below 0 the first.  F is the
+// type numpy plans in: double, or float for a float32 array (q / float32(100), then (n - 1) * q, both in float32).
+template <typename F> struct PctPlanOf { int prev, next; F gamma; };
+using PctPlan = PctPlanOf<double>;
 
-__host__ __device__ inline PctPlan pct_plan(int n, double q_percent) {
-    const double vi = (double)(n - 1) * (q_percent / 100.0);
-    PctPlan p;
-    if (vi >= (double)(n - 1)) {
+template <typename F>
+__host__ __device__ inline PctPlanOf<F> pct_plan(int n, F q_percent) {
+    const F vi = (F)(n - 1) * (q_percent / (F)100.0);
+    PctPlanOf<F> p;
+    if (vi >= (F)(n - 1)) {
         p.prev = p.next = n - 1;
         p.gamma = 0.0;
-    } else if (vi < 0.0) {
+    } else if (vi < (F)0.0) {
         p.prev = p.next = 0;
         p.gamma = 0.0;
     } else {
-        const double prev = floor(vi);
+        const F prev = floor(vi);
         p.prev = (int)prev;
         p.next = p.prev + 1;
         p.gamma = vi - prev;
@@ -65,13 +68,14 @@ __host__ __device__ inline PctPlan pct_plan(int n, double q_percent) {
 }
 
 // numpy _lerp (numpy/lib/_function_base_impl.py): a + (b-a)*t, and b - (b-a)*(1-t) where t >= 0.5; with pct_plan the two halves of
-// np.percentile(method="linear")
-__host__ __device__ __forceinline__ double np_lerp(double a, double b, double t) {
-    const double d = b - a;
-    double r = a + d * t;
-    if (t >= 0.5) r = b - d * (1.0 - t);
+// np.percentile(method="linear").  np_lerp_d takes d = b - a as numpy formed it: an integer array subtracts in its own type.
+template <typename F>
+__host__ __device__ __forceinline__ F np_lerp_d(F a, F b, F d, F t) {
+    F r = a + d * t;
+    if (t >= (F)0.5) r = b - d * ((F)1.0 - t);
     return r;
 }
+__host__ __device__ __forceinline__ double np_lerp(double a, double b, double t) { return np_lerp_d(a, b, b - a, t); }
 
 int make_stats_geom(StatsGeom* g, int H, int W);
 

@@ -25,6 +25,11 @@ from .core.utilities import ResultBase, ResultsDataMixin
 from .core.warnings import capture_warnings
 
 
+def percent_integral_uniformity(max: float, min: float) -> float:
+    """planar_imaging.py:140-143: 100 * (1 - (max - min + 1e-6) / (max + min + 1e-6)); the constant keeps a blank disk finite."""
+    return 100 * (1 - (max - min + 1e-6) / (max + min + 1e-6))
+
+
 class LightRadResult(ResultBase):
     """planar_imaging.py:1169-1198"""
 
