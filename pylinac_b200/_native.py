@@ -1017,9 +1017,7 @@ def nm_fov(ctx: Context, binary: np.ndarray, erode: float) -> tuple[np.ndarray, 
 def nt_slices(ctx: Context, volumes, nz: int, ufov_erode: float) -> np.ndarray:
     """epid_nt_slices on uint16 volumes (Batch of n x nz slices, or ndarray [n, nz, h, w]) -> one NT_SLICE_DTYPE row per slice,
     [n * nz]"""
-    if not isinstance(volumes, Batch):
-        volumes = np.ascontiguousarray(volumes).reshape(-1, *np.shape(volumes)[-2:])
-    with batch_for(ctx, volumes, np.uint16) as b:
+    with batch_for(ctx, _volume_batch(volumes), np.uint16) as b:
         (n, _, _), _ = b.shape_dtype
         res = np.zeros(n, NT_SLICE_DTYPE)
         _unsupported_as_not_implemented(lib().epid_nt_slices(ctx.handle, b.handle, int(nz), float(ufov_erode), _ptr(res)))
@@ -1029,10 +1027,8 @@ def nt_slices(ctx: Context, volumes, nz: int, ufov_erode: float) -> np.ndarray:
 def nt_spheres(ctx: Context, volumes, nz: int, spheres: np.ndarray, maxfun: int = 600, maxiter: int = 600) -> np.ndarray:
     """epid_nt_spheres: the sphere searches of `spheres` (NT_SPHERE_IN_DTYPE rows) in uint16 volumes (Batch of n x nz slices, or
     ndarray [n, nz, h, w]) -> one NT_SPHERE_DTYPE row per sphere"""
-    if not isinstance(volumes, Batch):
-        volumes = np.ascontiguousarray(volumes).reshape(-1, *np.shape(volumes)[-2:])
     spheres = np.ascontiguousarray(spheres, NT_SPHERE_IN_DTYPE)
-    with batch_for(ctx, volumes, np.uint16) as b:
+    with batch_for(ctx, _volume_batch(volumes), np.uint16) as b:
         res = np.zeros(len(spheres), NT_SPHERE_DTYPE)
         _unsupported_as_not_implemented(lib().epid_nt_spheres(ctx.handle, b.handle, int(nz), _ptr(spheres), len(spheres), int(maxfun),
                                                               int(maxiter), _ptr(res)))

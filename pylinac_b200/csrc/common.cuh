@@ -41,6 +41,9 @@ inline size_t dtype_size(int dt) {
     return 0;
 }
 
+// b bytes rounded up to a multiple of 256 (the alignment of each buffer carved out of a scratch area)
+inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
 }  // namespace epid
 
 struct epid_ctx {

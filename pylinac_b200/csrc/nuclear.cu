@@ -10,11 +10,9 @@
 //
 // Exactness (DESIGN.md section 4.14): every filtered value is S / 16 with S an integer, so the threshold mean, the Michelson ratios
 // and the EDT comparison are evaluated on exact integers and round once, as numpy does.
-#include "ccl.cuh"
 #include "common.cuh"
 #include "nuclear_stages.cuh"
 
-#include <climits>
 #include <cmath>
 
 namespace epid {
@@ -25,7 +23,6 @@ using namespace nm;
 constexpr int NM_BIN_THREADS = 256;
 constexpr int NM_BIN_COLS = 2048;      // raw columns per pass of k_nm_bin (a multiple of every supported bin)
 constexpr int NM_THREADS = 512;
-constexpr int NM_MAX_BIN = 64;         // 16 * 65535 * 64^2 < 2^32: S stays a uint32
 
 // block sums of bin x bin raw pixels for binned row blockIdx.x of frame blockIdx.y.  Each thread sums raw columns over the bin's rows
 // (coalesced along the row), then each binned column adds its bin column sums.  VEC: w % 8 == 0, 16-byte loads of 8 pixels.
@@ -79,16 +76,16 @@ struct NmPlanes {                 // optional device outputs of k_nm_frame (null
 };
 
 // FULL: `in` holds block sums and the frame is filtered, thresholded and cleaned first.  !FULL (get_fov): `in` is the frame's binary.
+// ws: the global workspace, 12 bytes per pixel per frame; nullptr: the frame is in dynamic shared memory.
 template <typename TIn, bool FULL>
 __global__ void __launch_bounds__(NM_THREADS) k_nm_frame(const TIn* __restrict__ in, int hb, int wb, double ufov_erode, double cfov_erode,
-                                                         int win, double thr_frac, int use_smem, uint32_t* ws, epid_nm_result* res,
-                                                         NmPlanes out) {
+                                                         int win, double thr_frac, uint32_t* ws, epid_nm_result* res, NmPlanes out) {
     extern __shared__ __align__(16) uint32_t dsm[];
     __shared__ unsigned long long red[32];
     const int f = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
     const int N = hb * wb;
     const size_t fo = (size_t)f * N;
-    uint32_t* S = use_smem ? dsm : ws + 3 * fo;
+    uint32_t* S = ws ? ws + 3 * fo : dsm;
     int* P = (int*)(S + N);       // -1 / union-find parent; later the squared EDT
     int* A = (int*)(S + 2 * N);   // component areas; later the column distances of the EDT
     const TIn* B = in + fo;
@@ -130,27 +127,19 @@ __global__ void __launch_bounds__(NM_THREADS) k_nm_frame(const TIn* __restrict__
         for (int p = tid; p < N; p += nt)
             if ((double)S[p] * 0.0625 < thr) S[p] = 0;
         __syncthreads();
-        // ---- remove_small_objects(min_size=2), connectivity 1: a foreground pixel without a 4-neighbour in the foreground goes
-        for (int p = tid; p < N; p += nt) {
-            const int i = p / wb, j = p - i * wb;
-            const bool nb = (i > 0 && S[p - wb]) || (i < hb - 1 && S[p + wb]) || (j > 0 && S[p - 1]) || (j < wb - 1 && S[p + 1]);
-            P[p] = S[p] && nb ? p : -1;
-        }
-        __syncthreads();
-        for (int p = tid; p < N; p += nt) {
-            if (P[p] < 0) S[p] = 0;
-            if (out.clean_s) out.clean_s[fo + p] = S[p];
-            if (out.cleaned) out.cleaned[fo + p] = (double)S[p] * 0.0625;
-        }
+        remove_stray_pixels(S, P, hb, wb, [&](int p, uint32_t s) {
+            if (out.clean_s) out.clean_s[fo + p] = s;
+            if (out.cleaned) out.cleaned[fo + p] = (double)s * 0.0625;
+        });
     } else {
         __syncthreads();
         for (int p = tid; p < N; p += nt) P[p] = S[p] ? p : -1;
+        __syncthreads();
     }
-    __syncthreads();
 
     label_areas(P, A, hb, wb);
-    const int longest = largest_longest(P, A, hb, wb, red);
-    if (longest == 0) {           // no component: get_fov's max() over no regions raises
+    const int longest = largest_component(P, A, hb, wb, red).longest;
+    if (longest == 0) {           // no component (area and longest 0): get_fov's max() over no regions raises
         if (tid == 0) {
             r.status = EPID_NM_NO_COMPONENT;
             res[f] = r;
@@ -167,60 +156,30 @@ __global__ void __launch_bounds__(NM_THREADS) k_nm_frame(const TIn* __restrict__
     if (tid == 0) res[f] = r;
 }
 
-size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
-struct NmScratch {
-    uint32_t* binned = nullptr;
-    epid_nm_result* res = nullptr;
-    uint32_t* ws = nullptr;
-    int use_smem = 0;
-    size_t smem = 0;
-};
-
-// lays out ctx->scratch: [binned sums (full)] [result rows] [per-frame workspace when the frame does not fit shared memory] [extra]
-int nm_scratch(epid_ctx* ctx, int n, int hb, int wb, bool full, size_t extra, NmScratch* s, char** extra_ptr) {
+// ctx->scratch: [binned sums (full)] [result rows] [per-frame workspace when the frame does not fit shared memory] [extra]
+int nm_scratch(epid_ctx* ctx, int n, int hb, int wb, bool full, size_t extra, FrameScratch* s) {
     const size_t N = (size_t)hb * wb;
-    int optin = 0;
-    EPID_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
-    s->smem = 12 * N;
-    s->use_smem = s->smem + 1024 <= (size_t)optin;
-    const size_t b_bin = full ? align256(N * n * sizeof(uint32_t)) : 0;
-    const size_t b_res = align256(n * sizeof(epid_nm_result));
-    const size_t b_ws = s->use_smem ? 0 : align256(12 * N * n);
-    int rc = ensure_scratch(ctx, b_bin + b_res + b_ws + extra);
-    if (rc != EPID_OK) return rc;
-    char* base = (char*)ctx->scratch;
-    s->binned = full ? (uint32_t*)base : nullptr;
-    s->res = (epid_nm_result*)(base + b_bin);
-    s->ws = s->use_smem ? nullptr : (uint32_t*)(base + b_bin + b_res);
-    if (extra_ptr) *extra_ptr = base + b_bin + b_res + b_ws;
-    if (!s->use_smem) s->smem = 0;
-    return EPID_OK;
+    return frame_scratch(ctx, n, N, 12, 1024, full ? N * n * sizeof(uint32_t) : 0, n * sizeof(epid_nm_result), extra, s);
 }
 
 int nm_check(const epid_batch* frames, int bin, int window, int* hb, int* wb) {
-    EPID_REQUIRE(frames, EPID_ERR_INVALID, "NULL argument");
-    EPID_REQUIRE(frames->dtype == EPID_U16, EPID_ERR_UNSUPPORTED, "nuclear frames must be uint16 (dtype %d)", frames->dtype);
-    EPID_REQUIRE(bin >= 1 && bin <= NM_MAX_BIN && (bin & (bin - 1)) == 0, EPID_ERR_UNSUPPORTED,
-                 "bin size %d: expected a power of two up to %d", bin, NM_MAX_BIN);
-    EPID_REQUIRE(window >= 1, EPID_ERR_INVALID, "window size %d < 1", window);
-    *hb = (frames->h + bin - 1) / bin;
-    *wb = (frames->w + bin - 1) / bin;
-    EPID_REQUIRE((long long)*hb * *wb < (1LL << 30), EPID_ERR_UNSUPPORTED, "binned frame %d x %d is too large", *hb, *wb);
-    return EPID_OK;
+    int rc = check_volumes(frames, 1, "nuclear frames");
+    return rc != EPID_OK ? rc : check_binning(frames, bin, window, 1LL << 30, hb, wb);
 }
 
-int nm_launch(epid_ctx* ctx, const epid_batch* frames, int bin, double ue, double ce, int window, double thr, const NmScratch& s, int hb,
+int nm_launch(epid_ctx* ctx, const epid_batch* frames, int bin, double ue, double ce, int window, double thr, const FrameScratch& s, int hb,
               int wb, const NmPlanes& planes) {
     const int n = frames->n;
     const dim3 bgrid(hb, n);
+    uint32_t* binned = (uint32_t*)s.head;
     if (frames->w % 8 == 0)
-        k_nm_bin<true><<<bgrid, NM_BIN_THREADS, 0, ctx->stream>>>((const uint16_t*)frames->dptr, frames->h, frames->w, bin, hb, wb, s.binned);
+        k_nm_bin<true><<<bgrid, NM_BIN_THREADS, 0, ctx->stream>>>((const uint16_t*)frames->dptr, frames->h, frames->w, bin, hb, wb, binned);
     else
-        k_nm_bin<false><<<bgrid, NM_BIN_THREADS, 0, ctx->stream>>>((const uint16_t*)frames->dptr, frames->h, frames->w, bin, hb, wb, s.binned);
+        k_nm_bin<false><<<bgrid, NM_BIN_THREADS, 0, ctx->stream>>>((const uint16_t*)frames->dptr, frames->h, frames->w, bin, hb, wb, binned);
     EPID_CUDA(cudaGetLastError());
     EPID_SMEM_OPT_IN(ctx, (k_nm_frame<uint32_t, true>), s.smem);
-    k_nm_frame<uint32_t, true><<<n, NM_THREADS, s.smem, ctx->stream>>>(s.binned, hb, wb, ue, ce, window, thr, s.use_smem, s.ws, s.res, planes);
+    k_nm_frame<uint32_t, true><<<n, NM_THREADS, s.smem, ctx->stream>>>(binned, hb, wb, ue, ce, window, thr, (uint32_t*)s.ws,
+                                                                       (epid_nm_result*)s.rows, planes);
     EPID_CUDA(cudaGetLastError());
     ctx->launches += 2;
     return EPID_OK;
@@ -239,8 +198,8 @@ extern "C" int32_t epid_nm_uniformity(epid_ctx* ctx, const epid_batch* frames, i
     int rc = nm_check(frames, bin, window, &hb, &wb);
     if (rc != EPID_OK) return rc;
     EPID_CUDA(cudaSetDevice(ctx->device));
-    NmScratch s;
-    if ((rc = nm_scratch(ctx, frames->n, hb, wb, true, 0, &s, nullptr)) != EPID_OK) return rc;
+    FrameScratch s;
+    if ((rc = nm_scratch(ctx, frames->n, hb, wb, true, 0, &s)) != EPID_OK) return rc;
     NmPlanes planes = {};
     epid_batch *bc = nullptr, *bm = nullptr;
     if (cleaned) {
@@ -254,14 +213,8 @@ extern "C" int32_t epid_nm_uniformity(epid_ctx* ctx, const epid_batch* frames, i
         }
         planes.masks = (uint8_t*)bm->dptr;
     }
-    rc = nm_launch(ctx, frames, bin, ufov_erode, cfov_erode, window, threshold, s, hb, wb, planes);
-    cudaError_t e = rc == EPID_OK ? cudaMemcpyAsync(results, s.res, frames->n * sizeof(epid_nm_result), cudaMemcpyDeviceToHost, ctx->stream)
-                                  : cudaSuccess;
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (rc == EPID_OK && e != cudaSuccess) {
-        set_error("nuclear uniformity failed: %s", cudaGetErrorString(e));
-        rc = EPID_ERR_CUDA;
-    }
+    if ((rc = nm_launch(ctx, frames, bin, ufov_erode, cfov_erode, window, threshold, s, hb, wb, planes)) == EPID_OK)
+        rc = finish(ctx, results, s.rows, frames->n * sizeof(epid_nm_result), "nuclear uniformity");
     if (rc != EPID_OK) {
         epid_batch_free(bc);
         epid_batch_free(bm);
@@ -282,18 +235,17 @@ extern "C" int32_t epid_nm_stages(epid_ctx* ctx, const epid_batch* frames, int32
     EPID_CUDA(cudaSetDevice(ctx->device));
     const size_t plane = (size_t)frames->n * hb * wb;
     const size_t b4 = align256(4 * plane);
-    NmScratch s;
-    char* extra = nullptr;
-    if ((rc = nm_scratch(ctx, frames->n, hb, wb, true, 3 * b4 + align256(2 * plane), &s, &extra)) != EPID_OK) return rc;
+    FrameScratch s;
+    if ((rc = nm_scratch(ctx, frames->n, hb, wb, true, 3 * b4 + align256(2 * plane), &s)) != EPID_OK) return rc;
     NmPlanes planes = {};
-    planes.filtered = (uint32_t*)extra;
-    planes.clean_s = (uint32_t*)(extra + b4);
-    planes.edt2 = (int32_t*)(extra + 2 * b4);
-    planes.masks = (uint8_t*)(extra + 3 * b4);
+    planes.filtered = (uint32_t*)s.extra;
+    planes.clean_s = (uint32_t*)(s.extra + b4);
+    planes.edt2 = (int32_t*)(s.extra + 2 * b4);
+    planes.masks = (uint8_t*)(s.extra + 3 * b4);
     EPID_CUDA(cudaMemsetAsync(planes.edt2, 0xff, 4 * plane, ctx->stream));    // -1 where a frame stops before its EDT
     EPID_CUDA(cudaMemsetAsync(planes.masks, 0, 2 * plane, ctx->stream));
     if ((rc = nm_launch(ctx, frames, bin, ufov_erode, cfov_erode, window, threshold, s, hb, wb, planes)) != EPID_OK) return rc;
-    EPID_CUDA(cudaMemcpyAsync(results, s.res, frames->n * sizeof(epid_nm_result), cudaMemcpyDeviceToHost, ctx->stream));
+    EPID_CUDA(cudaMemcpyAsync(results, s.rows, frames->n * sizeof(epid_nm_result), cudaMemcpyDeviceToHost, ctx->stream));
     EPID_CUDA(cudaMemcpyAsync(filtered, planes.filtered, 4 * plane, cudaMemcpyDeviceToHost, ctx->stream));
     EPID_CUDA(cudaMemcpyAsync(cleaned, planes.clean_s, 4 * plane, cudaMemcpyDeviceToHost, ctx->stream));
     EPID_CUDA(cudaMemcpyAsync(edt2, planes.edt2, 4 * plane, cudaMemcpyDeviceToHost, ctx->stream));
@@ -308,26 +260,19 @@ extern "C" int32_t epid_nm_fov(epid_ctx* ctx, const epid_batch* binary, double e
     EPID_REQUIRE((long long)binary->h * binary->w < (1LL << 30), EPID_ERR_UNSUPPORTED, "frame %d x %d is too large", binary->h, binary->w);
     EPID_CUDA(cudaSetDevice(ctx->device));
     const int n = binary->n, hb = binary->h, wb = binary->w;
-    NmScratch s;
-    int rc = nm_scratch(ctx, n, hb, wb, false, align256(2 * (size_t)n * hb * wb), &s, nullptr);
+    FrameScratch s;
+    int rc = nm_scratch(ctx, n, hb, wb, false, align256(2 * (size_t)n * hb * wb), &s);
     if (rc != EPID_OK) return rc;
     epid_batch* bm = nullptr;
     if ((rc = epid_batch_alloc(ctx, EPID_U8, 2 * n, hb, wb, &bm)) != EPID_OK) return rc;
     NmPlanes planes = {};
     planes.masks = (uint8_t*)bm->dptr;
-    cudaError_t e = cudaSuccess;
     rc = smem_opt_in(ctx, k_nm_frame<uint8_t, false>, s.smem);
     if (rc == EPID_OK) {
         k_nm_frame<uint8_t, false><<<n, NM_THREADS, s.smem, ctx->stream>>>((const uint8_t*)binary->dptr, hb, wb, erode, erode, 1, 0.0,
-                                                                           s.use_smem, s.ws, s.res, planes);
+                                                                           (uint32_t*)s.ws, (epid_nm_result*)s.rows, planes);
         ctx->launches += 1;
-        e = cudaGetLastError();
-        if (e == cudaSuccess) e = cudaMemcpyAsync(results, s.res, n * sizeof(epid_nm_result), cudaMemcpyDeviceToHost, ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-        if (e != cudaSuccess) {
-            set_error("nuclear FOV failed: %s", cudaGetErrorString(e));
-            rc = EPID_ERR_CUDA;
-        }
+        rc = finish(ctx, results, s.rows, n * sizeof(epid_nm_result), "nuclear FOV");
     }
     if (rc != EPID_OK) {
         epid_batch_free(bm);

@@ -1,19 +1,66 @@
 // The frame stages of get_fov and the FOV uniformities (pylinac.nuclear, nuclear.py:158-271 and 457-481) shared by k_nm_frame
-// (nuclear.cu) and k_tu_frame (nuclear_tu.cu).  Every stage runs on a whole CTA over one frame of hb x wb pixels held in two int
-// planes P and A (shared memory or a global workspace) and decides on `value > 0` only, so it is the same for integer and float64
-// frames.  Each function ends with the CTA synchronised.
+// (nuclear.cu), k_tu_frame (nuclear_tu.cu) and k_nt_slices (nuclear_tomo.cu), and the host code around those kernels.  Every stage
+// runs on a whole CTA over one frame of hb x wb pixels held in two int planes P and A (shared memory or a global workspace) and
+// decides on `value > 0` only, so it is the same for integer and float64 frames.  Each stage ends with the CTA synchronised.
 #pragma once
 
 #include <climits>
 #include <cmath>
 
 #include "ccl.cuh"
-#include "nuclear_reduce.cuh"
+#include "common.cuh"
 
 namespace epid {
 namespace nm {
 
 constexpr int NM_BIG = 1 << 20;        // column distance of a pixel with no background above / below it
+// the largest bin: 16 * 65535 * 64^2 < 2^32 keeps k_nm_frame's S a uint32, and each of k_tu_bin's rows stays one pairwise leaf
+constexpr int NM_MAX_BIN = 64;
+
+struct OpMax {
+    template <class T>
+    __device__ T operator()(T a, T b) const { return a > b ? a : b; }
+};
+struct OpMin {
+    template <class T>
+    __device__ T operator()(T a, T b) const { return a < b ? a : b; }
+};
+struct OpSum {
+    template <class T>
+    __device__ T operator()(T a, T b) const { return a + b; }
+};
+
+// block-wide reduction of a 64-bit value; every thread gets the result
+template <class T, class Op>
+__device__ T block_reduce(T v, Op op, unsigned long long* red) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v = op(v, (T)__shfl_xor_sync(0xffffffffu, (unsigned long long)v, o));
+    __syncthreads();                                        // red[] may still be read by the previous reduction
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = (unsigned long long)v;
+    __syncthreads();
+    T r = (T)red[0];
+    for (int k = 1; k < (int)(blockDim.x >> 5); k++) r = op(r, (T)red[k]);
+    return r;
+}
+
+// remove_small_objects(min_size=2), connectivity 1: a foreground pixel (value > 0) without a 4-neighbour in the foreground goes.  On
+// exit P[p] is p for a kept pixel and -1 otherwise, and val[p] is 0 where P[p] is -1; emit(p, val[p]) sees each pixel's final value.
+template <class V, class Emit>
+__device__ __forceinline__ void remove_stray_pixels(V* val, int* P, int hb, int wb, Emit emit) {
+    const int N = hb * wb, tid = threadIdx.x, nt = blockDim.x;
+    for (int p = tid; p < N; p += nt) {
+        const int i = p / wb, j = p - i * wb;
+        const bool nb = (i > 0 && val[p - wb] > 0) || (i < hb - 1 && val[p + wb] > 0) || (j > 0 && val[p - 1] > 0) ||
+                        (j < wb - 1 && val[p + 1] > 0);
+        P[p] = val[p] > 0 && nb ? p : -1;
+    }
+    __syncthreads();
+    for (int p = tid; p < N; p += nt) {
+        if (P[p] < 0) val[p] = 0;
+        emit(p, val[p]);
+    }
+    __syncthreads();
+}
 
 // 4-connected labelling of the foreground (P[p] = p, background -1 on entry): on exit P[p] is the component's root, the smallest index
 // of the component (skimage's raster label order), and A[root] its area.
@@ -36,9 +83,15 @@ __device__ __forceinline__ void label_areas(int* P, int* A, int hb, int wb) {
     __syncthreads();
 }
 
-// the largest component (on ties the lowest label, i.e. the smallest root) and the longer side of its bounding box; 0 when there is
-// no component (get_fov's max() over no regions raises)
-__device__ __forceinline__ int largest_longest(const int* P, const int* A, int hb, int wb, unsigned long long* red) {
+struct Component {
+    int root;                        // the smallest index of the component
+    int area;                        // 0: there is no component
+    int longest;                     // the longer side of its bounding box
+    unsigned long long rsum, csum;   // the exact sums of its pixels' row and column indices
+};
+
+// the largest component, on ties the lowest label, i.e. the smallest root (Python's max() keeps the first)
+__device__ __forceinline__ Component largest_component(const int* P, const int* A, int hb, int wb, unsigned long long* red) {
     const int N = hb * wb, tid = threadIdx.x, nt = blockDim.x;
     unsigned long long key = 0;
     for (int p = tid; p < N; p += nt) {
@@ -47,22 +100,30 @@ __device__ __forceinline__ int largest_longest(const int* P, const int* A, int h
         key = k > key ? k : key;
     }
     key = block_reduce(key, OpMax(), red);
-    if (key == 0) return 0;
-    const int root = (int)(0xffffffffu - (uint32_t)key);
+    Component c = {};
+    if (key == 0) return c;
+    c.root = (int)(0xffffffffu - (uint32_t)key);
+    c.area = (int)(key >> 32);
     long long rmin = LLONG_MAX, rmax = -1, cmin = LLONG_MAX, cmax = -1;
+    unsigned long long rsum = 0, csum = 0;
     for (int p = tid; p < N; p += nt) {
-        if (P[p] != root) continue;
+        if (P[p] != c.root) continue;
         const int i = p / wb, j = p - i * wb;
         rmin = min(rmin, (long long)i);
         rmax = max(rmax, (long long)i);
         cmin = min(cmin, (long long)j);
         cmax = max(cmax, (long long)j);
+        rsum += i;
+        csum += j;
     }
     rmin = block_reduce(rmin, OpMin(), red);
     rmax = block_reduce(rmax, OpMax(), red);
     cmin = block_reduce(cmin, OpMin(), red);
     cmax = block_reduce(cmax, OpMax(), red);
-    return (int)max(rmax - rmin + 1, cmax - cmin + 1);
+    c.rsum = block_reduce(rsum, OpSum(), red);
+    c.csum = block_reduce(csum, OpSum(), red);
+    c.longest = (int)max(rmax - rmin + 1, cmax - cmin + 1);
+    return c;
 }
 
 // exact squared EDT of the whole binary frame (P >= 0: foreground): column distances into A, then the row-wise minimum of
@@ -229,6 +290,66 @@ __device__ __forceinline__ void fov_uniformity(const V* val, const int* edt2, co
             }
         }
     }
+}
+
+// ------------------------------------------------------------------------------------------------ host side of the frame kernels
+
+// uint16 frames, read as volumes of nz slices each; `what` names them in the dtype error
+inline int check_volumes(const epid_batch* b, int nz, const char* what) {
+    EPID_REQUIRE(b, EPID_ERR_INVALID, "NULL argument");
+    EPID_REQUIRE(b->dtype == EPID_U16, EPID_ERR_UNSUPPORTED, "%s must be uint16 (dtype %d)", what, b->dtype);
+    EPID_REQUIRE(nz >= 1 && b->n % nz == 0, EPID_ERR_INVALID, "%d slices do not divide the batch's %d frames", nz, b->n);
+    return EPID_OK;
+}
+
+// the bin size and uniformity window of the FOV uniformities; *hb x *wb: the binned frame, fewer than max_pixels
+inline int check_binning(const epid_batch* b, int bin, int window, long long max_pixels, int* hb, int* wb) {
+    EPID_REQUIRE(bin >= 1 && bin <= NM_MAX_BIN && (bin & (bin - 1)) == 0, EPID_ERR_UNSUPPORTED,
+                 "bin size %d: expected a power of two up to %d", bin, NM_MAX_BIN);
+    EPID_REQUIRE(window >= 1, EPID_ERR_INVALID, "window size %d < 1", window);
+    *hb = (b->h + bin - 1) / bin;
+    *wb = (b->w + bin - 1) / bin;
+    EPID_REQUIRE((long long)*hb * *wb < max_pixels, EPID_ERR_UNSUPPORTED, "binned frame %d x %d is too large", *hb, *wb);
+    return EPID_OK;
+}
+
+struct FrameScratch {
+    char* head;       // the caller's leading buffer
+    char* rows;       // the result rows
+    char* ws;         // the per-frame workspace; nullptr: each CTA holds its frame in `smem` bytes of dynamic shared memory
+    char* extra;      // the caller's trailing buffers
+    size_t smem;
+};
+
+// Lays out ctx->scratch as [head] [rows] [workspace] [extra] for a kernel that runs one CTA per frame of N pixels at bpp bytes per
+// pixel.  The frame goes to dynamic shared memory when it fits beside static_smem bytes of static shared memory, else to a workspace
+// of bpp x N bytes per frame.  head, rows and the workspace are each rounded up to 256 bytes.
+inline int frame_scratch(epid_ctx* ctx, int n, size_t N, size_t bpp, size_t static_smem, size_t head, size_t rows, size_t extra,
+                         FrameScratch* s) {
+    int optin = 0;
+    EPID_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+    const bool fits = bpp * N + static_smem <= (size_t)optin;
+    const size_t b_head = align256(head), b_rows = align256(rows), b_ws = fits ? 0 : align256(bpp * N * n);
+    int rc = ensure_scratch(ctx, b_head + b_rows + b_ws + extra);
+    if (rc != EPID_OK) return rc;
+    s->head = (char*)ctx->scratch;
+    s->rows = s->head + b_head;
+    s->ws = fits ? nullptr : s->rows + b_rows;
+    s->extra = s->rows + b_rows + b_ws;
+    s->smem = fits ? bpp * N : 0;
+    return EPID_OK;
+}
+
+// the end of an entry point: check the launches, copy the result rows to the host and wait for them
+inline int finish(epid_ctx* ctx, void* dst, const void* src, size_t bytes, const char* what) {
+    cudaError_t e = cudaGetLastError();
+    if (e == cudaSuccess) e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
+    if (e != cudaSuccess) {
+        set_error("%s failed: %s", what, cudaGetErrorString(e));
+        return EPID_ERR_CUDA;
+    }
+    return EPID_OK;
 }
 
 }  // namespace nm

@@ -3,20 +3,19 @@
 //
 //   k_nt_max      one CTA per volume: the volume's maximum.
 //   k_nt_slices   one CTA per slice, the slice in shared memory when 12 bytes per pixel fit (the global workspace otherwise; same
-//                 code): the threshold at 10 % of the volume's maximum (compared in float64, as numpy promotes it), 4-connected
-//                 labelling with the largest region's area, bounding box and exact coordinate sums, one exact squared EDT of the whole
-//                 binary against erosion / 2, and the Michelson ratio, exact sum and count of the eroded pixels.
+//                 code): the threshold at 10 % of the volume's maximum (compared in float64, as numpy promotes it), then the stages of
+//                 nuclear_stages.cuh shared with k_nm_frame and k_tu_frame: 4-connected labelling, the largest region's area, bounding
+//                 box and exact coordinate sums, and one exact squared EDT of the whole binary; the FOV against erosion / 2, and the
+//                 Michelson ratio, exact sum and count of the eroded pixels.
 //   k_nt_spheres  one CTA per (volume, sphere): scipy's _minimize_neldermead (nuclear_tomo.cuh), each objective evaluation an exact
 //                 sum and count over the sphere's bounding box, then the sum, count and min at res.x.
 //
 // Exactness (DESIGN.md section 4.15): the volumes are integer counts, so every sum is an exact integer below 2^53, every mean and
 // ratio rounds once, and the search's arithmetic is scipy's expression order without FMA (-fmad=false).
-#include "ccl.cuh"
 #include "common.cuh"
-#include "nuclear_reduce.cuh"
+#include "nuclear_stages.cuh"
 #include "nuclear_tomo.cuh"
 
-#include <climits>
 #include <cmath>
 
 namespace epid {
@@ -26,7 +25,6 @@ using namespace nm;
 
 constexpr int NT_THREADS = 512;
 constexpr int NT_SPHERE_THREADS = 128;
-constexpr int NT_BIG = 1 << 20;           // column distance of a pixel with no background above / below it
 
 __global__ void __launch_bounds__(NT_THREADS) k_nt_max(const uint16_t* __restrict__ vol, size_t voxels, uint32_t* __restrict__ gmax) {
     __shared__ unsigned long long red[32];
@@ -38,14 +36,14 @@ __global__ void __launch_bounds__(NT_THREADS) k_nt_max(const uint16_t* __restric
 }
 
 __global__ void __launch_bounds__(NT_THREADS) k_nt_slices(const uint16_t* __restrict__ vol, int nz, int h, int w,
-                                                          const uint32_t* __restrict__ gmax, double ufov_erode, int use_smem, uint32_t* ws,
+                                                          const uint32_t* __restrict__ gmax, double ufov_erode, uint32_t* ws,
                                                           epid_nt_slice* res) {
     extern __shared__ __align__(16) uint32_t dsm[];
     __shared__ unsigned long long red[32];
     const int f = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
     const int N = h * w;
     const size_t fo = (size_t)f * N;
-    uint32_t* S = use_smem ? dsm : ws + 3 * fo;
+    uint32_t* S = ws ? ws + 3 * fo : dsm;
     int* P = (int*)(S + N);       // -1 / union-find parent; later the squared EDT
     int* A = (int*)(S + 2 * N);   // component areas; later the column distances of the EDT
     const uint16_t* src = vol + fo;
@@ -57,97 +55,24 @@ __global__ void __launch_bounds__(NT_THREADS) k_nt_slices(const uint16_t* __rest
         const uint32_t v = src[p];
         S[p] = (double)v < thr ? 0u : v;
         P[p] = S[p] ? p : -1;
-        A[p] = 0;
     }
     __syncthreads();
 
-    // ---- 4-connected labelling: roots are the smallest index of their component (skimage's raster label order)
-    for (int p = tid; p < N; p += nt) {
-        if (P[p] < 0) continue;
-        const int i = p / w, j = p - i * w;
-        if (j > 0 && P[p - 1] >= 0) gl_union(P, p, p - 1);
-        if (i > 0 && P[p - w] >= 0) gl_union(P, p, p - w);
-    }
-    __syncthreads();
-    for (int p = tid; p < N; p += nt)
-        if (P[p] >= 0) P[p] = gl_find(P, p);
-    __syncthreads();
-    for (int p = tid; p < N; p += nt)
-        if (P[p] >= 0) atomicAdd(&A[P[p]], 1);
-    __syncthreads();
-    // the largest area; on ties the lowest label, i.e. the smallest root index (Python's max() keeps the first)
-    unsigned long long key = 0;
-    for (int p = tid; p < N; p += nt) {
-        if (P[p] != p) continue;
-        const unsigned long long k = ((unsigned long long)A[p] << 32) | (0xffffffffu - (uint32_t)p);
-        key = k > key ? k : key;
-    }
-    key = block_reduce(key, OpMax(), red);
-    if (key == 0) {               // no label: slice_data skips the slice
+    label_areas(P, A, h, w);
+    const Component c = largest_component(P, A, h, w, red);
+    if (c.area == 0) {            // no label: slice_data skips the slice
         if (tid == 0) {
             r.status = EPID_NT_NO_COMPONENT;
             res[f] = r;
         }
         return;
     }
-    const int root = (int)(0xffffffffu - (uint32_t)key);
-    const long long npix = (long long)(key >> 32);
-    long long rmin = LLONG_MAX, rmax = -1, cmin = LLONG_MAX, cmax = -1;
-    unsigned long long rsum = 0, csum = 0;
-    for (int p = tid; p < N; p += nt) {
-        if (P[p] != root) continue;
-        const int i = p / w, j = p - i * w;
-        rmin = min(rmin, (long long)i);
-        rmax = max(rmax, (long long)i);
-        cmin = min(cmin, (long long)j);
-        cmax = max(cmax, (long long)j);
-        rsum += i;
-        csum += j;
-    }
-    rmin = block_reduce(rmin, OpMin(), red);
-    rmax = block_reduce(rmax, OpMax(), red);
-    cmin = block_reduce(cmin, OpMin(), red);
-    cmax = block_reduce(cmax, OpMax(), red);
-    rsum = block_reduce(rsum, OpSum(), red);
-    csum = block_reduce(csum, OpSum(), red);
-    const int longest = (int)max(rmax - rmin + 1, cmax - cmin + 1);
-    const int erosion = (int)rint(ufov_erode * (double)longest);    // int(round(...)): Python rounds halves to even, as rint does
-    r.longest = longest;
+    const int erosion = (int)rint(ufov_erode * (double)c.longest);  // int(round(...)): Python rounds halves to even, as rint does
+    r.longest = c.longest;
     r.erosion = erosion;
-    r.centroid_row = (double)rsum / (double)npix;                   // skimage: the mean of the global coordinates
-    r.centroid_col = (double)csum / (double)npix;
-
-    // ---- exact squared EDT of the whole binary slice: column distances, then the row-wise minimum of dk^2 + g^2
-    for (int j = tid; j < w; j += nt) {
-        int g = NT_BIG;
-        for (int i = 0; i < h; i++) {
-            const int p = i * w + j;
-            g = P[p] >= 0 ? min(g + 1, NT_BIG) : 0;
-            A[p] = g;
-        }
-        g = NT_BIG;
-        for (int i = h - 1; i >= 0; i--) {
-            const int p = i * w + j;
-            g = P[p] >= 0 ? min(g + 1, NT_BIG) : 0;
-            A[p] = min(A[p], g);
-        }
-    }
-    __syncthreads();
-    for (int p = tid; p < N; p += nt) {      // each thread reads and writes only its own P[p]
-        if (P[p] < 0) {
-            P[p] = 0;
-        } else {
-            const int i = p / w, j = p - i * w;
-            const int* g = A + (size_t)i * w;
-            long long best = (long long)g[j] * g[j];
-            for (int k = 1; (long long)k * k < best && (j - k >= 0 || j + k < w); k++) {
-                if (j - k >= 0) best = min(best, (long long)k * k + (long long)g[j - k] * g[j - k]);
-                if (j + k < w) best = min(best, (long long)k * k + (long long)g[j + k] * g[j + k]);
-            }
-            P[p] = (int)min(best, (long long)INT_MAX);
-        }
-    }
-    __syncthreads();
+    r.centroid_row = (double)c.rsum / (double)c.area;               // skimage: the mean of the global coordinates
+    r.centroid_col = (double)c.csum / (double)c.area;
+    squared_edt(P, A, h, w, nullptr);
 
     // ---- the FOV: distance > erosion / 2  <=>  4 d^2 > erosion^2 (every pixel when the erosion is negative)
     const long long e2 = (long long)erosion * erosion;
@@ -233,25 +158,11 @@ __global__ void __launch_bounds__(NT_SPHERE_THREADS) k_nt_spheres(const uint16_t
     }
 }
 
-size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 int nt_check(const epid_batch* volumes, int nz) {
-    EPID_REQUIRE(volumes, EPID_ERR_INVALID, "NULL argument");
-    EPID_REQUIRE(volumes->dtype == EPID_U16, EPID_ERR_UNSUPPORTED, "tomographic volumes must be uint16 (dtype %d)", volumes->dtype);
-    EPID_REQUIRE(nz >= 1 && volumes->n % nz == 0, EPID_ERR_INVALID, "%d slices do not divide the batch's %d frames", nz, volumes->n);
+    int rc = check_volumes(volumes, nz, "tomographic volumes");
+    if (rc != EPID_OK) return rc;
     EPID_REQUIRE((long long)volumes->h * volumes->w < (1LL << 28), EPID_ERR_UNSUPPORTED, "slice %d x %d is too large", volumes->h,
                  volumes->w);
-    return EPID_OK;
-}
-
-int finish(epid_ctx* ctx, void* dst, const void* src, size_t bytes, const char* what) {
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, ctx->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (e != cudaSuccess) {
-        set_error("%s failed: %s", what, cudaGetErrorString(e));
-        return EPID_ERR_CUDA;
-    }
     return EPID_OK;
 }
 
@@ -268,23 +179,17 @@ extern "C" int32_t epid_nt_slices(epid_ctx* ctx, const epid_batch* volumes, int3
     const int n = volumes->n, h = volumes->h, w = volumes->w, nvol = n / nz;
     if (n == 0) return EPID_OK;
     const size_t N = (size_t)h * w;
-    int optin = 0;
-    EPID_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
-    size_t smem = 12 * N;
-    const int use_smem = smem + 1024 <= (size_t)optin;
-    const size_t b_max = align256(nvol * sizeof(uint32_t)), b_res = align256(n * sizeof(epid_nt_slice));
-    if ((rc = ensure_scratch(ctx, b_max + b_res + (use_smem ? 0 : 12 * N * n))) != EPID_OK) return rc;
-    char* base = (char*)ctx->scratch;
-    uint32_t* gmax = (uint32_t*)base;
-    epid_nt_slice* res = (epid_nt_slice*)(base + b_max);
-    uint32_t* ws = use_smem ? nullptr : (uint32_t*)(base + b_max + b_res);
-    if (!use_smem) smem = 0;
+    // ctx->scratch: [volume maxima] [result rows] [per-slice workspace when the slice does not fit shared memory]
+    FrameScratch s;
+    if ((rc = frame_scratch(ctx, n, N, 12, 1024, nvol * sizeof(uint32_t), n * sizeof(epid_nt_slice), 0, &s)) != EPID_OK) return rc;
+    uint32_t* gmax = (uint32_t*)s.head;
     k_nt_max<<<nvol, NT_THREADS, 0, ctx->stream>>>((const uint16_t*)volumes->dptr, (size_t)nz * N, gmax);
     EPID_CUDA(cudaGetLastError());
-    EPID_SMEM_OPT_IN(ctx, k_nt_slices, smem);
-    k_nt_slices<<<n, NT_THREADS, smem, ctx->stream>>>((const uint16_t*)volumes->dptr, nz, h, w, gmax, ufov_erode, use_smem, ws, res);
+    EPID_SMEM_OPT_IN(ctx, k_nt_slices, s.smem);
+    k_nt_slices<<<n, NT_THREADS, s.smem, ctx->stream>>>((const uint16_t*)volumes->dptr, nz, h, w, gmax, ufov_erode, (uint32_t*)s.ws,
+                                                        (epid_nt_slice*)s.rows);
     ctx->launches += 2;
-    return finish(ctx, results, res, n * sizeof(epid_nt_slice), "tomographic slices");
+    return finish(ctx, results, s.rows, n * sizeof(epid_nt_slice), "tomographic slices");
 }
 
 extern "C" int32_t epid_nt_spheres(epid_ctx* ctx, const epid_batch* volumes, int32_t nz, const struct epid_nt_sphere_in* spheres,

@@ -6,7 +6,7 @@
 //               edges zero-padded: per block acc = 0; acc += pw(row) for each of its rows (skimage's block_reduce(func=np.sum)).
 //   k_tu_frame  one CTA per volume on the float64 binned frame, held in shared memory when 16 bytes per pixel fit (the global
 //               workspace otherwise; same code): convolve2d's order for the 9-point filter, edge zeroing, the threshold (the values
-//               above 10 % of the max compacted in raster order and their pairwise-sum mean), the stray-pixel stencil, then the
+//               above 10 % of the max compacted in raster order and their pairwise-sum mean), then the stray-pixel stencil and the
 //               stages of nuclear_stages.cuh shared with k_nm_frame for three FOVs (UFOV, CFOV, center), and the center and ring sums of
 //               center_border_ratio as pairwise sums over the whole frame.
 //
@@ -27,7 +27,6 @@ constexpr int TU_BIN_THREADS = 256;
 constexpr int TU_TILE = 4096;          // doubles of k_tu_bin's mean tile: bin raw rows x TU_TILE / bin raw columns
 constexpr int TU_THREADS = 512;
 constexpr int TU_LOG_THREADS = 9;
-constexpr int TU_MAX_BIN = 64;
 constexpr size_t TU_STATIC_SMEM = 8192;   // red[], wsum[] and slots[] of k_tu_frame, rounded up
 
 __global__ void __launch_bounds__(TU_BIN_THREADS) k_tu_bin(const uint16_t* __restrict__ vol, int nz, int h, int w, int first, int count,
@@ -79,8 +78,8 @@ struct TuPlanes {                 // optional device outputs of k_tu_frame (null
 };
 
 __global__ void __launch_bounds__(TU_THREADS) k_tu_frame(const double* __restrict__ binned, int hb, int wb, double ufov_erode,
-                                                         double cfov_erode, double center_erode, int win, double thr_frac, int use_smem,
-                                                         double* ws, epid_tu_result* res, TuPlanes out) {
+                                                         double cfov_erode, double center_erode, int win, double thr_frac, double* ws,
+                                                         epid_tu_result* res, TuPlanes out) {
     extern __shared__ __align__(16) double tsm[];
     __shared__ unsigned long long red[32];
     __shared__ int wsum[32];
@@ -88,7 +87,7 @@ __global__ void __launch_bounds__(TU_THREADS) k_tu_frame(const double* __restric
     const int f = blockIdx.x, tid = threadIdx.x, nt = blockDim.x;
     const int N = hb * wb;
     const size_t fo = (size_t)f * N;
-    double* M = use_smem ? tsm : ws + 2 * fo;
+    double* M = ws ? ws + 2 * fo : tsm;
     int* P = (int*)(M + N);       // -1 / union-find parent; later the squared EDT
     int* A = P + N;               // component areas; later the column distances of the EDT
     double* SEL = (double*)P;     // the threshold selection in raster order, before the stencil
@@ -142,21 +141,12 @@ __global__ void __launch_bounds__(TU_THREADS) k_tu_frame(const double* __restric
     for (int p = tid; p < N; p += nt)
         if (M[p] < thr) M[p] = 0.0;
     __syncthreads();
-    // ---- remove_small_objects(min_size=2), connectivity 1: a foreground pixel without a 4-neighbour in the foreground goes
-    for (int p = tid; p < N; p += nt) {
-        const int i = p / wb, j = p - i * wb;
-        const bool nb = (i > 0 && M[p - wb] > 0) || (i < hb - 1 && M[p + wb] > 0) || (j > 0 && M[p - 1] > 0) || (j < wb - 1 && M[p + 1] > 0);
-        P[p] = M[p] > 0 && nb ? p : -1;
-    }
-    __syncthreads();
-    for (int p = tid; p < N; p += nt) {
-        if (P[p] < 0) M[p] = 0.0;
-        if (out.cleaned) out.cleaned[fo + p] = M[p];
-    }
-    __syncthreads();
+    remove_stray_pixels(M, P, hb, wb, [&](int p, double m) {
+        if (out.cleaned) out.cleaned[fo + p] = m;
+    });
 
     label_areas(P, A, hb, wb);
-    const int longest = largest_longest(P, A, hb, wb, red);
+    const int longest = largest_component(P, A, hb, wb, red).longest;
     if (longest == 0) {           // no component: get_fov's max() over no regions raises
         if (tid == 0) {
             r.status = EPID_NM_NO_COMPONENT;
@@ -189,61 +179,30 @@ __global__ void __launch_bounds__(TU_THREADS) k_tu_frame(const double* __restric
     if (tid == 0) res[f] = r;
 }
 
-size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
-struct TuScratch {
-    double* binned = nullptr;
-    epid_tu_result* res = nullptr;
-    double* ws = nullptr;
-    int use_smem = 0;
-    size_t smem = 0;
-};
-
-// lays out ctx->scratch: [binned frames] [result rows] [per-volume workspace when the frame does not fit shared memory] [extra]
-int tu_scratch(epid_ctx* ctx, int nvol, int hb, int wb, size_t extra, TuScratch* s, char** extra_ptr) {
+// ctx->scratch: [binned frames] [result rows] [per-volume workspace when the frame does not fit shared memory] [extra]
+int tu_scratch(epid_ctx* ctx, int nvol, int hb, int wb, size_t extra, FrameScratch* s) {
     const size_t N = (size_t)hb * wb;
-    int optin = 0;
-    EPID_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
-    s->smem = 16 * N;
-    s->use_smem = s->smem + TU_STATIC_SMEM <= (size_t)optin;
-    const size_t b_bin = align256(8 * N * nvol);
-    const size_t b_res = align256(nvol * sizeof(epid_tu_result));
-    const size_t b_ws = s->use_smem ? 0 : align256(16 * N * nvol);
-    int rc = ensure_scratch(ctx, b_bin + b_res + b_ws + extra);
-    if (rc != EPID_OK) return rc;
-    char* base = (char*)ctx->scratch;
-    s->binned = (double*)base;
-    s->res = (epid_tu_result*)(base + b_bin);
-    s->ws = s->use_smem ? nullptr : (double*)(base + b_bin + b_res);
-    if (extra_ptr) *extra_ptr = base + b_bin + b_res + b_ws;
-    if (!s->use_smem) s->smem = 0;
-    return EPID_OK;
+    return frame_scratch(ctx, nvol, N, 16, TU_STATIC_SMEM, 8 * N * nvol, nvol * sizeof(epid_tu_result), extra, s);
 }
 
 int tu_check(const epid_batch* volumes, int nz, int first, int count, int bin, int window, int* hb, int* wb) {
-    EPID_REQUIRE(volumes, EPID_ERR_INVALID, "NULL argument");
-    EPID_REQUIRE(volumes->dtype == EPID_U16, EPID_ERR_UNSUPPORTED, "tomographic volumes must be uint16 (dtype %d)", volumes->dtype);
-    EPID_REQUIRE(nz >= 1 && volumes->n % nz == 0, EPID_ERR_INVALID, "%d slices do not divide the batch's %d frames", nz, volumes->n);
+    int rc = check_volumes(volumes, nz, "tomographic volumes");
+    if (rc != EPID_OK) return rc;
     EPID_REQUIRE(first >= 0 && count >= 1 && (long long)first + count <= nz, EPID_ERR_INVALID, "slab [%d, %d + %d) of %d slices", first,
                  first, count, nz);
-    EPID_REQUIRE(bin >= 1 && bin <= TU_MAX_BIN && (bin & (bin - 1)) == 0, EPID_ERR_UNSUPPORTED,
-                 "bin size %d: expected a power of two up to %d", bin, TU_MAX_BIN);
-    EPID_REQUIRE(window >= 1, EPID_ERR_INVALID, "window size %d < 1", window);
-    *hb = (volumes->h + bin - 1) / bin;
-    *wb = (volumes->w + bin - 1) / bin;
-    EPID_REQUIRE((long long)*hb * *wb < (1LL << 28), EPID_ERR_UNSUPPORTED, "binned frame %d x %d is too large", *hb, *wb);
-    return EPID_OK;
+    return check_binning(volumes, bin, window, 1LL << 28, hb, wb);
 }
 
 int tu_launch(epid_ctx* ctx, const epid_batch* volumes, int nz, int first, int count, int bin, const double* erode, int window,
-              double thr, const TuScratch& s, int hb, int wb, double* mean, const TuPlanes& planes) {
+              double thr, const FrameScratch& s, int hb, int wb, double* mean, const TuPlanes& planes) {
     const int nvol = volumes->n / nz;
+    double* binned = (double*)s.head;
     k_tu_bin<<<dim3(hb, nvol), TU_BIN_THREADS, 0, ctx->stream>>>((const uint16_t*)volumes->dptr, nz, volumes->h, volumes->w, first, count,
-                                                                  bin, hb, wb, s.binned, mean);
+                                                                  bin, hb, wb, binned, mean);
     EPID_CUDA(cudaGetLastError());
     EPID_SMEM_OPT_IN(ctx, k_tu_frame, s.smem);
-    k_tu_frame<<<nvol, TU_THREADS, s.smem, ctx->stream>>>(s.binned, hb, wb, erode[0], erode[1], erode[2], window, thr, s.use_smem, s.ws,
-                                                          s.res, planes);
+    k_tu_frame<<<nvol, TU_THREADS, s.smem, ctx->stream>>>(binned, hb, wb, erode[0], erode[1], erode[2], window, thr, (double*)s.ws,
+                                                          (epid_tu_result*)s.rows, planes);
     EPID_CUDA(cudaGetLastError());
     ctx->launches += 2;
     return EPID_OK;
@@ -264,8 +223,8 @@ extern "C" int32_t epid_tu_uniformity(epid_ctx* ctx, const epid_batch* volumes, 
     const int nvol = volumes->n / nz;
     if (nvol == 0) return EPID_OK;
     EPID_CUDA(cudaSetDevice(ctx->device));
-    TuScratch s;
-    if ((rc = tu_scratch(ctx, nvol, hb, wb, 0, &s, nullptr)) != EPID_OK) return rc;
+    FrameScratch s;
+    if ((rc = tu_scratch(ctx, nvol, hb, wb, 0, &s)) != EPID_OK) return rc;
     TuPlanes planes = {};
     epid_batch *bmean = nullptr, *bc = nullptr, *bm = nullptr;
     auto release = [&]() {
@@ -286,14 +245,9 @@ extern "C" int32_t epid_tu_uniformity(epid_ctx* ctx, const epid_batch* volumes, 
     if (bm) planes.masks = (uint8_t*)bm->dptr;
     const double erode[3] = {ufov_erode, cfov_erode, center_erode};
     rc = tu_launch(ctx, volumes, nz, first, count, bin, erode, window, threshold, s, hb, wb, bmean ? (double*)bmean->dptr : nullptr, planes);
-    cudaError_t e = rc == EPID_OK ? cudaMemcpyAsync(results, s.res, nvol * sizeof(epid_tu_result), cudaMemcpyDeviceToHost, ctx->stream)
-                                  : cudaSuccess;
-    if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-    if (rc == EPID_OK && e != cudaSuccess) {
-        set_error("tomographic uniformity failed: %s", cudaGetErrorString(e));
-        rc = EPID_ERR_CUDA;
-    }
+    if (rc == EPID_OK) rc = finish(ctx, results, s.rows, nvol * sizeof(epid_tu_result), "tomographic uniformity");
     if (rc != EPID_OK) {
+        cudaStreamSynchronize(ctx->stream);   // k_tu_bin may still be writing the slab means when k_tu_frame failed to launch
         release();
         return rc;
     }
@@ -316,22 +270,21 @@ extern "C" int32_t epid_tu_stages(epid_ctx* ctx, const epid_batch* volumes, int3
     EPID_CUDA(cudaSetDevice(ctx->device));
     const size_t plane = (size_t)nvol * hb * wb, raw = (size_t)nvol * volumes->h * volumes->w;
     const size_t b8 = align256(8 * plane), b4 = align256(4 * plane), b_mean = align256(8 * raw);
-    TuScratch s;
-    char* extra = nullptr;
-    if ((rc = tu_scratch(ctx, nvol, hb, wb, b_mean + 2 * b8 + b4 + align256(3 * plane), &s, &extra)) != EPID_OK) return rc;
-    double* dmean = (double*)extra;
+    FrameScratch s;
+    if ((rc = tu_scratch(ctx, nvol, hb, wb, b_mean + 2 * b8 + b4 + align256(3 * plane), &s)) != EPID_OK) return rc;
+    double* dmean = (double*)s.extra;
     TuPlanes planes = {};
-    planes.filtered = (double*)(extra + b_mean);
-    planes.cleaned = (double*)(extra + b_mean + b8);
-    planes.edt2 = (int32_t*)(extra + b_mean + 2 * b8);
-    planes.masks = (uint8_t*)(extra + b_mean + 2 * b8 + b4);
+    planes.filtered = (double*)(s.extra + b_mean);
+    planes.cleaned = (double*)(s.extra + b_mean + b8);
+    planes.edt2 = (int32_t*)(s.extra + b_mean + 2 * b8);
+    planes.masks = (uint8_t*)(s.extra + b_mean + 2 * b8 + b4);
     EPID_CUDA(cudaMemsetAsync(planes.edt2, 0xff, 4 * plane, ctx->stream));    // -1 where a frame stops before its EDT
     EPID_CUDA(cudaMemsetAsync(planes.masks, 0, 3 * plane, ctx->stream));
     const double erode[3] = {ufov_erode, cfov_erode, center_erode};
     if ((rc = tu_launch(ctx, volumes, nz, first, count, bin, erode, window, threshold, s, hb, wb, dmean, planes)) != EPID_OK) return rc;
-    EPID_CUDA(cudaMemcpyAsync(results, s.res, nvol * sizeof(epid_tu_result), cudaMemcpyDeviceToHost, ctx->stream));
+    EPID_CUDA(cudaMemcpyAsync(results, s.rows, nvol * sizeof(epid_tu_result), cudaMemcpyDeviceToHost, ctx->stream));
     EPID_CUDA(cudaMemcpyAsync(mean, dmean, 8 * raw, cudaMemcpyDeviceToHost, ctx->stream));
-    EPID_CUDA(cudaMemcpyAsync(binned, s.binned, 8 * plane, cudaMemcpyDeviceToHost, ctx->stream));
+    EPID_CUDA(cudaMemcpyAsync(binned, s.head, 8 * plane, cudaMemcpyDeviceToHost, ctx->stream));
     EPID_CUDA(cudaMemcpyAsync(filtered, planes.filtered, 8 * plane, cudaMemcpyDeviceToHost, ctx->stream));
     EPID_CUDA(cudaMemcpyAsync(cleaned, planes.cleaned, 8 * plane, cudaMemcpyDeviceToHost, ctx->stream));
     EPID_CUDA(cudaMemcpyAsync(edt2, planes.edt2, 4 * plane, cudaMemcpyDeviceToHost, ctx->stream));

@@ -575,7 +575,7 @@ extern "C" int32_t epid_roi_stats(epid_ctx* ctx, const epid_batch* b, int32_t nr
     int rc = ensure_scratch(ctx, nv + no + 512);
     if (rc != EPID_OK) return rc;
     double* d_verts = (double*)ctx->scratch;
-    RoiOut* d_out = (RoiOut*)((char*)ctx->scratch + (nv + 255) / 256 * 256);
+    RoiOut* d_out = (RoiOut*)((char*)ctx->scratch + align256(nv));
     EPID_CUDA(cudaMemcpyAsync(d_verts, verts_xy, nv, cudaMemcpyHostToDevice, ctx->stream));
     EPID_DISPATCH_ROI(b->dtype, do_roi, ctx, b, nroi, d_verts, d_out);
     if (rc != EPID_OK) return rc;
@@ -663,7 +663,7 @@ extern "C" int32_t epid_disk_stats(epid_ctx* ctx, const epid_batch* b, int32_t n
     rc = ensure_scratch(ctx, nd + no + 512);
     if (rc != EPID_OK) return rc;
     double* d_disks = (double*)ctx->scratch;
-    DiskOut* d_out = (DiskOut*)((char*)ctx->scratch + (nd + 255) / 256 * 256);
+    DiskOut* d_out = (DiskOut*)((char*)ctx->scratch + align256(nd));
     EPID_CUDA(cudaMemcpyAsync(d_disks, disks, nd, cudaMemcpyHostToDevice, ctx->stream));
     const size_t smem = sizeof(int) * (size_t)(2 * max_rows + 1);
     EPID_DISPATCH_ROI(b->dtype, do_disk, ctx, b, ndisk, d_disks, d_out, smem);
@@ -700,13 +700,12 @@ extern "C" int32_t epid_disk_percentiles(epid_ctx* ctx, const epid_batch* b, int
     EPID_CUDA(cudaSetDevice(ctx->device));
     const size_t nd = sizeof(double) * 4 * ndisk, nqb = sizeof(double) * nq, no = sizeof(double) * (size_t)ndisk * nq,
                  nc = sizeof(long long) * (size_t)ndisk;
-    auto up = [](size_t v) { return (v + 255) / 256 * 256; };
-    rc = ensure_scratch(ctx, up(nd) + up(nqb) + up(no) + nc + 256);
+    rc = ensure_scratch(ctx, align256(nd) + align256(nqb) + align256(no) + nc + 256);
     if (rc != EPID_OK) return rc;
     double* d_disks = (double*)ctx->scratch;
-    double* d_q = (double*)((char*)d_disks + up(nd));
-    double* d_out = (double*)((char*)d_q + up(nqb));
-    long long* d_count = (long long*)((char*)d_out + up(no));
+    double* d_q = (double*)((char*)d_disks + align256(nd));
+    double* d_out = (double*)((char*)d_q + align256(nqb));
+    long long* d_count = (long long*)((char*)d_out + align256(no));
     EPID_CUDA(cudaMemcpyAsync(d_disks, disks, nd, cudaMemcpyHostToDevice, ctx->stream));
     EPID_CUDA(cudaMemcpyAsync(d_q, q_percent, nqb, cudaMemcpyHostToDevice, ctx->stream));
     const size_t smem = sizeof(int) * (size_t)(2 * max_rows + 1);

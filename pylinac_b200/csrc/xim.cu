@@ -306,8 +306,6 @@ int launch_decode(epid_ctx* ctx, const uint8_t* d_arena, const XimFrame* d_frame
     return EPID_OK;
 }
 
-size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
 }  // namespace
 }  // namespace epid
 
