@@ -100,8 +100,9 @@ int32_t epid_frame_histogram(epid_ctx* ctx, const epid_batch* b, int32_t r0, int
 int32_t epid_invert(epid_ctx* ctx, const epid_batch* in, epid_batch** out);
 /* array_utils.bit_invert (core/array_utils.py:81-89): integer dtypes only, else EPID_ERR_INVALID */
 int32_t epid_bit_invert(epid_ctx* ctx, const epid_batch* in, epid_batch** out);
-/* array_utils.ground (core/array_utils.py:93-102): a - min + value, same dtype; mins: double[n] (may be NULL) */
-int32_t epid_ground(epid_ctx* ctx, const epid_batch* in, double value, epid_batch** out, double* mins);
+/* array_utils.ground (core/array_utils.py:93-102): a - min + value, same dtype (value must be integral for integer
+ * dtypes); mins (may be NULL): the n frame minima, in the batch's dtype */
+int32_t epid_ground(epid_ctx* ctx, const epid_batch* in, double value, epid_batch** out, void* mins);
 /* array_utils.normalize (core/array_utils.py:64-71): a / (value or max) -> F64; use_max != 0 ignores value */
 int32_t epid_normalize(epid_ctx* ctx, const epid_batch* in, int32_t use_max, double value, epid_batch** out);
 /* BaseImage.threshold (core/image.py:785-800): keep a >= t (kind 0, 'high') or a <= t (kind 1), else 0; same dtype */
@@ -111,7 +112,8 @@ int32_t epid_binarize(epid_ctx* ctx, const epid_batch* in, double t, epid_batch*
 
 /* ----------------------------------------------------------------------------------------- stencils */
 /* scipy.ndimage.median_filter(a, size=k) as called by array_utils.filter (core/array_utils.py:131):
- * full k x k footprint, mode='reflect', rank k*k/2, dtype preserved. */
+ * full k x k footprint, mode='reflect', rank k*k/2, dtype preserved; frames of one row: the k-wide window at rank k/2.
+ * EPID_ERR_UNSUPPORTED when the k-dependent tile exceeds the device's shared memory per block (DESIGN.md 4.7). */
 int32_t epid_median_filter(epid_ctx* ctx, const epid_batch* in, int32_t size, epid_batch** out);
 /* scipy.ndimage.gaussian_filter(a, sigma) as called by array_utils.filter (core/array_utils.py:133):
  * separable, axis 0 then axis 1, radius int(4*sigma+0.5), mode='reflect', float64 accumulate,

@@ -1,7 +1,12 @@
 """``pylinac.core.array_utils`` (core/array_utils.py:38-212) with the pixel arithmetic executed by libepid.so.
 
 Every function uploads the array to HBM, runs the CUDA operator with the reference's dtype semantics and
-downloads the result.  1-D arrays (profiles) are handled as a single row.  No numpy/scipy compute fallback.
+downloads the result.  1-D arrays (profiles) are handled as a single row; a 3-D array is a batch of frames, each
+processed as the 2-D call would process it alone.  No numpy/scipy compute fallback.
+
+Dtypes follow numpy 2: bool, int8 and uint32 give numpy's results and exceptions (int8 and uint32 compute in int16 /
+int64 and cast back modularly, which is exact for every operator here), and a scalar argument takes part in type
+promotion as numpy's weak Python scalars or strong numpy scalars do.  uint64 and float16 raise TypeError.
 """
 from __future__ import annotations
 
@@ -10,6 +15,9 @@ import ctypes as C
 import numpy as np
 
 from .. import _native as nat
+
+# dtypes the device computes in for the ones it has no kernels for (exact: modular for int8 / uint32, 0 / 1 for bool)
+_WIDEN = {np.dtype(np.bool_): np.dtype(np.uint8), np.dtype(np.int8): np.dtype(np.int16), np.dtype(np.uint32): np.dtype(np.int64)}
 
 
 def _ctx():
@@ -31,25 +39,25 @@ def _as3d(a: np.ndarray):
 
 def _coerce(a: np.ndarray) -> np.ndarray:
     a = np.ascontiguousarray(a)
-    if a.dtype == np.bool_:
-        a = a.astype(np.uint8)
     if a.dtype.byteorder == ">":
         a = a.astype(a.dtype.newbyteorder("<"))
-    if a.dtype == np.uint32:
-        a = a.astype(np.int64)
-    if a.dtype == np.int8:
-        a = a.astype(np.int16)
+    if a.dtype in _WIDEN:
+        a = a.astype(_WIDEN[a.dtype])
     if a.dtype not in nat._NP2DT:
         raise TypeError(f"dtype {a.dtype} is not supported by the native operators")
     return a
 
 
-def _run(a, fn, *args):
+def _run(a, fn, *args, same_dtype: bool = True):
+    """Run the unary operator on the device; ``same_dtype``: the result has the input's dtype (cast back from the widened one)."""
+    dt = np.asarray(a).dtype
     a = _coerce(a)
     a3, shape = _as3d(a)
     ctx = _ctx()
     with nat.Batch.upload(ctx, a3) as b, b._unary(fn, *args) as out:
         res = out.download()
+    if same_dtype and res.dtype != dt:
+        res = res.astype(dt.newbyteorder("="))
     if res.size == int(np.prod(shape)):
         return res.reshape(shape)
     # shape-changing operators (zoom): drop the batch / row axes the input did not have
@@ -68,13 +76,23 @@ def geometric_center_value(array: np.ndarray) -> float:  # :47-60
 
 
 def normalize(array: np.ndarray, value: float | None = None) -> np.ndarray:  # :64-71
+    """array / (value or array.max()) with numpy 2's result dtype: float32 for a float32 array over its own max or a Python
+    scalar, float64 when either side is float64 (an ``np.float64`` value included)."""
+    a = np.asarray(array)
     if value is None:
-        return _run(array, nat.lib().epid_normalize, 1, 0.0)
-    return _run(array, nat.lib().epid_normalize, 0, float(value))
+        return _run(a, nat.lib().epid_normalize, 1, 0.0, same_dtype=False)
+    rt = np.result_type(a.dtype, value)
+    if rt.kind in "f" and rt != a.dtype:
+        a = a.astype(rt)       # exact: numpy converts the array to the result dtype before dividing
+    return _run(a, nat.lib().epid_normalize, 0, float(value), same_dtype=False)
 
 
 def invert(array: np.ndarray) -> np.ndarray:  # :75-77
-    return _run(array, nat.lib().epid_invert)
+    a = np.asarray(array)
+    if a.dtype == np.bool_:
+        raise TypeError("The numpy boolean negative, the `-` operator, is not supported, use the `~` operator or the logical_not "
+                        "function instead.")
+    return _run(a, nat.lib().epid_invert)
 
 
 def bit_invert(array: np.ndarray) -> np.ndarray:  # :81-89
@@ -82,21 +100,37 @@ def bit_invert(array: np.ndarray) -> np.ndarray:  # :81-89
     if a.dtype.kind == "f":
         raise ValueError(f"The datatype {a.dtype} could not be safely inverted. This usually means the array is a float-like "
                          "datatype. Cast to an integer-like datatype first.")
-    return _run(array, nat.lib().epid_bit_invert)
+    if a.dtype == np.bool_:
+        return _run(a, nat.lib().epid_bit_invert, same_dtype=False) == 255      # ~0 = 255, ~1 = 254: np.invert is the logical not
+    return _run(a, nat.lib().epid_bit_invert)
 
 
 def ground_with_min(array: np.ndarray, value: float = 0):
-    a = _coerce(np.asarray(array))
+    """(array - array.min() + value, array.min()); the minimum is a scalar of the array's dtype (one per frame for a batch).
+    ``a - min`` is taken in the array's dtype (wrapping as numpy's does) and ``+ value`` in numpy 2's result dtype: the array's
+    own for an in-range Python int (out of range: numpy's OverflowError), a wider one for a float or a wider numpy scalar."""
+    a0 = np.asarray(array)
+    if a0.dtype == np.bool_:
+        raise TypeError("numpy boolean subtract, the `-` operator, is not supported, use the bitwise_xor, the `^` operator, or the "
+                        "logical_xor function instead.")
+    rt = np.result_type(a0.dtype, value)
+    same = rt == a0.dtype
+    if same and a0.dtype.kind in "iu":
+        a0.dtype.type(value)       # OverflowError for a Python int outside the dtype, as numpy's `+ value` raises
+    a = _coerce(a0)
     a3, shape = _as3d(a)
     ctx = _ctx()
-    mins = np.empty(a3.shape[0], np.float64)
+    mins = np.empty(a3.shape[0], a.dtype)
     h = C.c_void_p()
     with nat.Batch.upload(ctx, a3) as b:
-        nat.check(nat.lib().epid_ground(ctx.handle, b.handle, float(value), C.byref(h), mins.ctypes.data_as(C.c_void_p)))
+        nat.check(nat.lib().epid_ground(ctx.handle, b.handle, float(value) if same else 0.0, C.byref(h), mins.ctypes.data_as(C.c_void_p)))
         with nat.Batch(ctx, h) as out:
             res = out.download().reshape(shape)
-    mn = a.dtype.type(mins[0]) if a3.shape[0] == 1 else mins.astype(a.dtype)
-    return res, mn
+    dt = a0.dtype.newbyteorder("=")
+    res, mins = res.astype(dt, copy=False), mins.astype(dt)
+    if not same:
+        res = res + value          # numpy's promotion of the grounded array and the scalar (host-resident result)
+    return res, (mins[0] if a3.shape[0] == 1 else mins)
 
 
 def ground(array: np.ndarray, value: float = 0) -> np.ndarray:  # :93-102
@@ -104,9 +138,12 @@ def ground(array: np.ndarray, value: float = 0) -> np.ndarray:  # :93-102
 
 
 def filter(array: np.ndarray, size=0.05, kind: str = "median") -> np.ndarray:  # :106-138
+    """ndimage.median_filter(array, size) / ndimage.gaussian_filter(array, sigma=size) of a profile or frame; a float size is
+    that fraction of the rows (of each frame's rows for a batch)."""
     if isinstance(size, float):
         if 0 < size < 1:
-            size = int(round(len(array) * size))
+            rows = len(array) if np.ndim(array) < 3 else np.shape(array)[1]
+            size = int(round(rows * size))
             size = max(size, 1)
         else:
             raise ValueError("Float was passed but was not between 0 and 1")
@@ -128,6 +165,8 @@ def _gaussian_kernel1d(sigma: float, radius: int) -> np.ndarray:
 def gaussian_filter(array: np.ndarray, sigma: float, truncate: float = 4.0) -> np.ndarray:
     """scipy.ndimage.gaussian_filter(array, sigma) semantics (mode='reflect', per-pass cast to the input dtype)."""
     a = np.asarray(array)
+    if a.dtype == np.bool_:
+        raise TypeError("gaussian_filter of a bool array is not supported")
     sd = float(sigma)
     lw = int(truncate * sd + 0.5)
     w = np.ascontiguousarray(_gaussian_kernel1d(sd, lw)[::-1])
@@ -142,7 +181,8 @@ def zoom(array: np.ndarray, zoom: float, order: int = 3, mode: str = "constant",
         raise ValueError("zoom mode must be 'constant' or 'nearest'")
     if grid_mode and mode != "nearest":
         raise ValueError("grid_mode zoom is implemented for mode 'nearest'")
-    return _run(array, nat.lib().epid_zoom, float(zoom), int(order), (0 if mode == "constant" else 1) | (2 if grid_mode else 0))
+    return _run(array, nat.lib().epid_zoom, float(zoom), int(order), (0 if mode == "constant" else 1) | (2 if grid_mode else 0),
+                same_dtype=False)
 
 
 def rotate(array: np.ndarray, angle: float, mode: str = "edge") -> np.ndarray:
@@ -150,21 +190,43 @@ def rotate(array: np.ndarray, angle: float, mode: str = "edge") -> np.ndarray:
     images: uint8 / 255, uint16 / 65535) -> float64, on the device (csrc/zoom.cu)."""
     if mode not in ("edge", "constant"):
         raise ValueError("rotate mode must be 'edge' or 'constant'")
-    return _run(array, nat.lib().epid_rotate, float(angle), 1 if mode == "edge" else 0)
+    return _run(array, nat.lib().epid_rotate, float(angle), 1 if mode == "edge" else 0, same_dtype=False)
 
 
 def sobel(array: np.ndarray, axis: int = -1) -> np.ndarray:
-    return _run(array, nat.lib().epid_sobel, int(axis))
+    """ndimage.sobel(array, axis): the [-1, 0, 1] derivative along ``axis``, then [1, 2, 1] along the other axis of a frame.
+    A 1-D profile has no other axis: its result is the derivative alone."""
+    a = np.asarray(array)
+    if a.dtype == np.bool_:
+        raise TypeError("sobel of a bool array is not supported")
+    if a.ndim == 1:
+        if axis not in (0, -1):
+            raise ValueError("axis must be 0 or -1 for a 1-D array")
+        d = np.array([-1.0, 0.0, 1.0])
+        return _run(a, nat.lib().epid_correlate1d_passes, d.ctypes.data_as(C.c_void_p), 1, 2)
+    return _run(a, nat.lib().epid_sobel, int(axis))
+
+
+def _compare_threshold(a: np.ndarray, t) -> float:
+    """The threshold as the double that compares with every pixel as numpy 2's ``a >= t`` does: numpy compares in
+    np.result_type(a, t), which is float32 for a float32 array and a Python float, so t is rounded to float32 first (exact
+    comparisons of float32 pixels in double).  A wider result type compares exactly in double already."""
+    if np.result_type(a.dtype, t) == np.float32:
+        return float(np.float32(t))
+    return float(t)
 
 
 def threshold(array: np.ndarray, threshold: float, kind: str = "high") -> np.ndarray:
-    """np.where(a >= t, a, 0) / np.where(a <= t, a, 0)  (core/image.py:797-800)"""
-    return _run(array, nat.lib().epid_threshold, float(threshold), 0 if kind == "high" else 1)
+    """np.where(a >= t, a, 0) / np.where(a <= t, a, 0)  (core/image.py:797-800); int64 for a bool array, as np.where gives"""
+    a = np.asarray(array)
+    res = _run(a, nat.lib().epid_threshold, _compare_threshold(a, threshold), 0 if kind == "high" else 1, same_dtype=a.dtype != np.bool_)
+    return res.astype(np.int64) if a.dtype == np.bool_ else res
 
 
 def binarize(array: np.ndarray, threshold: float) -> np.ndarray:
     """np.where(a >= t, 1, 0) -> int64 (core/image.py:814)"""
-    return _run(array, nat.lib().epid_binarize, float(threshold))
+    a = np.asarray(array)
+    return _run(a, nat.lib().epid_binarize, _compare_threshold(a, threshold), same_dtype=False)
 
 
 def stretch(array: np.ndarray, min: int = 0, max: int = 1) -> np.ndarray:  # :142-168

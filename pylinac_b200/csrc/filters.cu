@@ -1,6 +1,18 @@
-// Shared-memory tiled stencils.  Median: scipy.ndimage.median_filter(a, size=k) as array_utils.filter calls it
-// (core/array_utils.py:131): full k x k footprint, mode='reflect', rank (k*k)/2 of the sorted window (the UPPER
-// median for even k), window offsets -(k/2) .. k-1-(k/2) on both axes, dtype preserved.
+// Shared-memory tiled stencils.
+//
+// Median: scipy.ndimage.median_filter(a, size=k) as array_utils.filter calls it (core/array_utils.py:131): full k x k
+// footprint, mode='reflect', rank (k*k)/2 of the sorted window (the UPPER median for even k), window offsets
+// -(k/2) .. k-1-(k/2) on both axes, dtype preserved.  Every dtype selects the rank the same way: bisection over an
+// order-preserving unsigned key (MedKey), counting the window elements <= mid at each step.  A frame of one row (a 1-D
+// profile, or a 2-D frame of height 1) runs k_median_row: its k x k window holds k copies of each of k samples, so rank
+// k*k/2 is rank k/2 of the k-wide row window.  Tiles are sized per call, (32 + k - 1) x (8 + k - 1) keys for frames and
+// 256 + k - 1 keys for rows, up to the device's opt-in shared memory per block; a size no tile can hold is refused.
+//
+// correlate1d: scipy's symmetric / anti-symmetric summation order in fp64, mode='reflect', per-pass cast to the input
+// dtype.  The weights live in device memory allocated for the call on the context's stream, so any radius runs and two
+// contexts on one device never share them.
+#include <type_traits>
+
 #include "filters.cuh"
 
 namespace epid {
@@ -17,6 +29,65 @@ __device__ __forceinline__ int reflect_idx(int i, int n) {
 }
 
 #define EPID_CSWAP(a, b) { const uint32_t _lo = min(a, b); b = max(a, b); a = _lo; }
+
+// Order-preserving unsigned keys: a < b (numpy's order; -0 before +0) <=> key(a) < key(b).  K is the tile element type,
+// MAX the largest key the dtype can produce (the bisection's upper bound: 8 steps for uint8, 64 for the 8-byte dtypes).
+template <typename T> struct MedKey;
+template <> struct MedKey<uint8_t> {
+    using K = uint16_t; static constexpr uint64_t MAX = 0xFF;
+    static __device__ __forceinline__ K key(uint8_t v) { return v; }
+    static __device__ __forceinline__ uint8_t val(uint64_t k) { return (uint8_t)k; }
+};
+template <> struct MedKey<uint16_t> {
+    using K = uint16_t; static constexpr uint64_t MAX = 0xFFFF;
+    static __device__ __forceinline__ K key(uint16_t v) { return v; }
+    static __device__ __forceinline__ uint16_t val(uint64_t k) { return (uint16_t)k; }
+};
+template <> struct MedKey<int16_t> {
+    using K = uint16_t; static constexpr uint64_t MAX = 0xFFFF;
+    static __device__ __forceinline__ K key(int16_t v) { return (uint16_t)v ^ 0x8000u; }
+    static __device__ __forceinline__ int16_t val(uint64_t k) { return (int16_t)(uint16_t)(k ^ 0x8000u); }
+};
+template <> struct MedKey<int32_t> {
+    using K = uint32_t; static constexpr uint64_t MAX = 0xFFFFFFFFull;
+    static __device__ __forceinline__ K key(int32_t v) { return (uint32_t)v ^ 0x80000000u; }
+    static __device__ __forceinline__ int32_t val(uint64_t k) { return (int32_t)((uint32_t)k ^ 0x80000000u); }
+};
+template <> struct MedKey<long long> {
+    using K = uint64_t; static constexpr uint64_t MAX = ~0ull;
+    static __device__ __forceinline__ K key(long long v) { return (uint64_t)v ^ 0x8000000000000000ull; }
+    static __device__ __forceinline__ long long val(uint64_t k) { return (long long)(k ^ 0x8000000000000000ull); }
+};
+template <> struct MedKey<float> {
+    using K = uint32_t; static constexpr uint64_t MAX = 0xFFFFFFFFull;
+    static __device__ __forceinline__ K key(float v) { const uint32_t b = __float_as_uint(v); return (b & 0x80000000u) ? ~b : (b | 0x80000000u); }
+    static __device__ __forceinline__ float val(uint64_t k) { const uint32_t b = (uint32_t)k; return __uint_as_float((b & 0x80000000u) ? (b & 0x7FFFFFFFu) : ~b); }
+};
+template <> struct MedKey<double> {
+    using K = uint64_t; static constexpr uint64_t MAX = ~0ull;
+    static __device__ __forceinline__ K key(double v) {
+        const uint64_t b = (uint64_t)__double_as_longlong(v);
+        return (b & 0x8000000000000000ull) ? ~b : (b | 0x8000000000000000ull);
+    }
+    static __device__ __forceinline__ double val(uint64_t k) {
+        return __longlong_as_double((long long)((k & 0x8000000000000000ull) ? (k & 0x7FFFFFFFFFFFFFFFull) : ~k));
+    }
+};
+
+// Smallest key v with #{window <= v} >= need, for the kh x kw window whose top-left element is win[0] (row stride tw).
+// C is the bisection's arithmetic type: 32 bits while the keys fit, 64 bits otherwise.
+template <typename C, typename K>
+__device__ __forceinline__ C rank_select(const K* win, int tw, int kh, int kw, int need, C hi) {
+    C lo = 0;
+    while (lo < hi) {
+        const C mid = lo + ((hi - lo) >> 1);
+        int c = 0;
+        for (int j = 0; j < kh; j++)
+            for (int i = 0; i < kw; i++) c += (win[j * tw + i] <= mid) ? 1 : 0;
+        if (c >= need) hi = mid; else lo = mid + 1;
+    }
+    return lo;
+}
 
 template <int K>
 __global__ void __launch_bounds__(MED_TW * MED_TH)
@@ -59,32 +130,110 @@ k_median_u16(const FrameRef* __restrict__ src, const FrameRef* __restrict__ dst,
         EPID_CSWAP(p[4], p[2]);
         result = p[4];
     } else {
-        // rank select by bisection on the 16 value bits: smallest v with #{window <= v} >= rank + 1
-        const int need = (k * k) / 2 + 1;
-        uint32_t lo = 0, hi = 65535;
-        while (lo < hi) {
-            const uint32_t mid = (lo + hi) >> 1;
-            int c = 0;
-            for (int j = 0; j < k; j++)
-                for (int i = 0; i < k; i++) c += (tile[(ly + j) * tw + lx + i] <= mid) ? 1 : 0;
-            if (c >= need) hi = mid; else lo = mid + 1;
-        }
-        result = lo;
+        result = rank_select<uint32_t>(tile + ly * tw + lx, tw, k, k, (k * k) / 2 + 1, 65535u);
     }
     const FrameRef d = dst[fi];
     const_cast<uint16_t*>(d.origin)[(size_t)y * d.pitch + x] = (uint16_t)result;
 }
 
+static constexpr size_t med_tile_bytes(size_t key_bytes, int k) { return key_bytes * (size_t)(MED_TW + k - 1) * (MED_TH + k - 1); }
+
+// The median tile must fit the opt-in shared memory of one block: refuse a size that does not, naming the limit.
+static int median_smem(epid_ctx* ctx, size_t smem, int k) {
+    int optin = 0;
+    EPID_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+    EPID_REQUIRE(smem <= (size_t)optin, EPID_ERR_UNSUPPORTED,
+                 "median filter size %d needs a %zu-byte shared-memory tile; the device allows %d bytes per block", k, smem, optin);
+    return EPID_OK;
+}
+
 int launch_median_u16(epid_ctx* ctx, cudaStream_t stream, const FrameRef* d_src, const FrameRef* d_dst, const ValueMap* d_maps,
                       const int* d_select, int n, int H, int W, int k) {
-    EPID_REQUIRE(k >= 1 && k <= 31, EPID_ERR_UNSUPPORTED, "median filter size %d outside 1..31", k);
+    EPID_REQUIRE(k >= 1, EPID_ERR_INVALID, "median filter size %d must be >= 1", k);
     dim3 grid((W + MED_TW - 1) / MED_TW, (H + MED_TH - 1) / MED_TH, n);
-    const size_t smem = sizeof(uint16_t) * (size_t)(MED_TW + k - 1) * (MED_TH + k - 1);
-    if (k == 3)
+    const size_t smem = med_tile_bytes(sizeof(uint16_t), k);
+    if (k == 3) {
         k_median_u16<3><<<grid, MED_TW * MED_TH, smem, stream>>>(d_src, d_dst, d_maps, d_select, H, W, k);
-    else
+    } else {
+        int rc = median_smem(ctx, smem, k);
+        if (rc != EPID_OK) return rc;
+        EPID_SMEM_OPT_IN(ctx, k_median_u16<0>, smem);
         k_median_u16<0><<<grid, MED_TW * MED_TH, smem, stream>>>(d_src, d_dst, d_maps, d_select, H, W, k);
+    }
     ctx->launches += 1;
+    EPID_CUDA(cudaGetLastError());
+    return EPID_OK;
+}
+
+// k x k median of compact frames (every dtype but uint16, which runs k_median_u16)
+template <typename T>
+__global__ void __launch_bounds__(MED_TW * MED_TH)
+k_median_key(const T* __restrict__ in, T* __restrict__ out, int H, int W, int k) {
+    using M = MedKey<T>;
+    using K = typename M::K;
+    using C = typename std::conditional<sizeof(K) <= 4, uint32_t, uint64_t>::type;
+    extern __shared__ __align__(8) unsigned char med_raw[];
+    K* tile = reinterpret_cast<K*>(med_raw);
+    const int fi = blockIdx.z;
+    const T* f = in + (size_t)fi * H * W;
+    const int off = k / 2;
+    const int tw = MED_TW + k - 1, th = MED_TH + k - 1;
+    const int x0 = blockIdx.x * MED_TW, y0 = blockIdx.y * MED_TH;
+    for (int i = threadIdx.x; i < tw * th; i += blockDim.x) {
+        const int ty = i / tw, tx = i - ty * tw;
+        tile[i] = M::key(f[(size_t)reflect_idx(y0 + ty - off, H) * W + reflect_idx(x0 + tx - off, W)]);
+    }
+    __syncthreads();
+    const int lx = threadIdx.x % MED_TW, ly = threadIdx.x / MED_TW;
+    const int x = x0 + lx, y = y0 + ly;
+    if (x >= W || y >= H) return;
+    out[(size_t)fi * H * W + (size_t)y * W + x] = M::val(rank_select<C>(tile + ly * tw + lx, tw, k, k, (k * k) / 2 + 1, (C)M::MAX));
+}
+
+// median of frames of one row: rank k/2 of the k-wide window (every dtype)
+constexpr int MED_ROW = 256;
+template <typename T>
+__global__ void __launch_bounds__(MED_ROW)
+k_median_row(const T* __restrict__ in, T* __restrict__ out, int W, int k) {
+    using M = MedKey<T>;
+    using K = typename M::K;
+    using C = typename std::conditional<sizeof(K) <= 4, uint32_t, uint64_t>::type;
+    extern __shared__ __align__(8) unsigned char med_raw[];
+    K* tile = reinterpret_cast<K*>(med_raw);
+    const T* f = in + (size_t)blockIdx.z * W;
+    const int x0 = blockIdx.x * MED_ROW;
+    for (int i = threadIdx.x; i < MED_ROW + k - 1; i += MED_ROW) tile[i] = M::key(f[reflect_idx(x0 + i - k / 2, W)]);
+    __syncthreads();
+    const int x = x0 + threadIdx.x;
+    if (x >= W) return;
+    out[(size_t)blockIdx.z * W + x] = M::val(rank_select<C>(tile + threadIdx.x, 0, 1, k, k / 2 + 1, (C)M::MAX));
+}
+
+template <typename T>
+static int run_median(epid_ctx* ctx, const epid_batch* in, epid_batch* out, int k) {
+    using K = typename MedKey<T>::K;
+    int rc;
+    if (in->h == 1) {
+        const size_t smem = sizeof(K) * ((size_t)MED_ROW + k - 1);
+        if ((rc = median_smem(ctx, smem, k)) != EPID_OK) return rc;
+        EPID_SMEM_OPT_IN(ctx, k_median_row<T>, smem);
+        k_median_row<T><<<dim3((in->w + MED_ROW - 1) / MED_ROW, 1, in->n), MED_ROW, smem, ctx->stream>>>((const T*)in->dptr, (T*)out->dptr, in->w, k);
+    } else if constexpr (std::is_same<T, uint16_t>::value) {
+        const int n = in->n;
+        if ((rc = ensure_scratch(ctx, 2 * sizeof(FrameRef) * n + 512)) != EPID_OK) return rc;
+        FrameRef* src = (FrameRef*)ctx->scratch;
+        FrameRef* dst = (FrameRef*)((char*)ctx->scratch + align256(sizeof(FrameRef) * n));
+        launch_refs_from_batch(ctx, ctx->stream, (const uint16_t*)in->dptr, n, in->h, in->w, 0, 0, src);
+        launch_refs_from_batch(ctx, ctx->stream, (const uint16_t*)out->dptr, n, in->h, in->w, 0, 0, dst);
+        return launch_median_u16(ctx, ctx->stream, src, dst, nullptr, nullptr, n, in->h, in->w, k);
+    } else {
+        const size_t smem = med_tile_bytes(sizeof(K), k);
+        if ((rc = median_smem(ctx, smem, k)) != EPID_OK) return rc;
+        EPID_SMEM_OPT_IN(ctx, k_median_key<T>, smem);
+        dim3 grid((in->w + MED_TW - 1) / MED_TW, (in->h + MED_TH - 1) / MED_TH, in->n);
+        k_median_key<T><<<grid, MED_TW * MED_TH, smem, ctx->stream>>>((const T*)in->dptr, (T*)out->dptr, in->h, in->w, k);
+    }
+    ctx->launches++;
     EPID_CUDA(cudaGetLastError());
     return EPID_OK;
 }
@@ -93,40 +242,6 @@ int launch_median_u16(epid_ctx* ctx, cudaStream_t stream, const FrameRef* d_src,
 
 // ================================================================================================ generic dtypes
 namespace epid {
-
-// rank-by-counting median for any ordered dtype (used for everything that is not uint16): O(k^4) per pixel,
-// exact scipy semantics (element of rank k*k/2 in the sorted window).
-template <typename T>
-__global__ void __launch_bounds__(MED_TW * MED_TH)
-k_median_generic(const T* __restrict__ in, T* __restrict__ out, int H, int W, int k) {
-    extern __shared__ unsigned char traw[];
-    T* tile = reinterpret_cast<T*>(traw);
-    const int fi = blockIdx.z;
-    const T* f = in + (size_t)fi * H * W;
-    const int off = k / 2;
-    const int tw = MED_TW + k - 1, th = MED_TH + k - 1;
-    const int x0 = blockIdx.x * MED_TW, y0 = blockIdx.y * MED_TH;
-    for (int i = threadIdx.x; i < tw * th; i += blockDim.x) {
-        const int ty = i / tw, tx = i - ty * tw;
-        tile[i] = f[(size_t)reflect_idx(y0 + ty - off, H) * W + reflect_idx(x0 + tx - off, W)];
-    }
-    __syncthreads();
-    const int lx = threadIdx.x % MED_TW, ly = threadIdx.x / MED_TW;
-    const int x = x0 + lx, y = y0 + ly;
-    if (x >= W || y >= H) return;
-    const int want = (k * k) / 2;
-    T result = tile[ly * tw + lx];
-    for (int a = 0; a < k * k; a++) {
-        const T v = tile[(ly + a / k) * tw + lx + a % k];
-        int rank = 0;
-        for (int b = 0; b < k * k; b++) {
-            const T o = tile[(ly + b / k) * tw + lx + b % k];
-            rank += (o < v || (o == v && b < a)) ? 1 : 0;
-        }
-        if (rank == want) { result = v; break; }
-    }
-    out[(size_t)fi * H * W + (size_t)y * W + x] = result;
-}
 
 // One 1-D correlation pass along `axis` with scipy.ndimage.correlate1d's symmetric / anti-symmetric summation
 // order (ni_filters.c NI_Correlate1D), mode='reflect', fp64 accumulation, result cast to T.
@@ -138,14 +253,14 @@ __device__ __forceinline__ T cast_from_double(double v) { return (T)v; }
 template <> __device__ __forceinline__ uint8_t cast_from_double<uint8_t>(double v) { return (uint8_t)(long long)v; }
 template <> __device__ __forceinline__ uint16_t cast_from_double<uint16_t>(double v) { return (uint16_t)(long long)v; }
 template <> __device__ __forceinline__ int16_t cast_from_double<int16_t>(double v) { return (int16_t)(long long)v; }
-template <> __device__ __forceinline__ int32_t cast_from_double<int32_t>(double v) { return (int32_t)(long long)v; }
-
-constexpr int CORR_MAX_TAPS = 513;
-__constant__ double c_weights[CORR_MAX_TAPS];
+// scipy's (npy_int)double is x86's cvttsd2si: a result outside int32 (or NaN) becomes INT32_MIN; narrower types wrap
+template <> __device__ __forceinline__ int32_t cast_from_double<int32_t>(double v) {
+    return (v >= -2147483648.0 && v < 2147483648.0) ? (int32_t)v : INT32_MIN;
+}
 
 template <typename T>
 __global__ void __launch_bounds__(256)
-k_correlate1d(const T* __restrict__ in, T* __restrict__ out, int H, int W, int axis, int r, int sym) {
+k_correlate1d(const T* __restrict__ in, T* __restrict__ out, const double* __restrict__ c_weights, int H, int W, int axis, int r, int sym) {
     const int fi = blockIdx.z;
     const T* f = in + (size_t)fi * H * W;
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
@@ -173,7 +288,6 @@ k_correlate1d(const T* __restrict__ in, T* __restrict__ out, int H, int W, int a
 
 template <typename T>
 static int run_correlate(epid_ctx* ctx, const void* in, void* out, int n, int H, int W, int axis, const double* w, int r) {
-    EPID_REQUIRE(2 * r + 1 <= CORR_MAX_TAPS, EPID_ERR_UNSUPPORTED, "kernel radius %d too large", r);
     // symmetry test as in scipy (ni_filters.c): |w[i] - w[2r-i]| <= DBL_EPSILON for all i -> symmetric
     int sym = 0;
     if (r > 0) {
@@ -184,22 +298,19 @@ static int run_correlate(epid_ctx* ctx, const void* in, void* out, int n, int H,
             for (int i = 1; i <= r; i++) if (fabs(w[r + i] + w[r - i]) > 2.220446049250313e-16) { sym = 0; break; }
         }
     }
-    EPID_CUDA(cudaMemcpyToSymbolAsync(c_weights, w, sizeof(double) * (2 * r + 1), 0, cudaMemcpyHostToDevice, ctx->stream));
-    dim3 grid((W + 255) / 256, H, n);
-    k_correlate1d<T><<<grid, 256, 0, ctx->stream>>>((const T*)in, (T*)out, H, W, axis, r, sym);
-    ctx->launches++;
-    EPID_CUDA(cudaGetLastError());
-    return EPID_OK;
-}
-
-template <typename T>
-static int run_median_generic(epid_ctx* ctx, const epid_batch* in, epid_batch* out, int k) {
-    dim3 grid((in->w + MED_TW - 1) / MED_TW, (in->h + MED_TH - 1) / MED_TH, in->n);
-    const size_t smem = sizeof(T) * (size_t)(MED_TW + k - 1) * (MED_TH + k - 1);
-    EPID_REQUIRE(smem <= 48 * 1024, EPID_ERR_UNSUPPORTED, "median filter size %d too large for this dtype", k);
-    k_median_generic<T><<<grid, MED_TW * MED_TH, smem, ctx->stream>>>((const T*)in->dptr, (T*)out->dptr, in->h, in->w, k);
-    ctx->launches++;
-    EPID_CUDA(cudaGetLastError());
+    // weights for this pass only, in stream order: a later pass or another context cannot overwrite them before the kernel reads them
+    double* d_w = nullptr;
+    EPID_CUDA(cudaMallocAsync((void**)&d_w, sizeof(double) * (2 * r + 1), ctx->stream));
+    cudaError_t e = cudaMemcpyAsync(d_w, w, sizeof(double) * (2 * r + 1), cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess) {
+        dim3 grid((W + 255) / 256, H, n);
+        k_correlate1d<T><<<grid, 256, 0, ctx->stream>>>((const T*)in, (T*)out, d_w, H, W, axis, r, sym);
+        ctx->launches++;
+        e = cudaGetLastError();
+    }
+    const cudaError_t ef = cudaFreeAsync(d_w, ctx->stream);
+    EPID_CUDA(e);
+    EPID_CUDA(ef);
     return EPID_OK;
 }
 
@@ -249,19 +360,7 @@ int32_t epid_median_filter(epid_ctx* ctx, const epid_batch* in, int32_t size, ep
     EPID_CUDA(cudaSetDevice(ctx->device));
     int rc = epid_batch_alloc(ctx, in->dtype, in->n, in->h, in->w, out);
     if (rc != EPID_OK) return rc;
-    if (in->dtype == EPID_U16) {
-        const int n = in->n;
-        rc = ensure_scratch(ctx, 2 * sizeof(FrameRef) * n + 512);
-        if (rc == EPID_OK) {
-            FrameRef* src = (FrameRef*)ctx->scratch;
-            FrameRef* dst = (FrameRef*)((char*)ctx->scratch + (sizeof(FrameRef) * n + 255) / 256 * 256);
-            launch_refs_from_batch(ctx, ctx->stream, (const uint16_t*)in->dptr, n, in->h, in->w, 0, 0, src);
-            launch_refs_from_batch(ctx, ctx->stream, (const uint16_t*)(*out)->dptr, n, in->h, in->w, 0, 0, dst);
-            rc = launch_median_u16(ctx, ctx->stream, src, dst, nullptr, nullptr, n, in->h, in->w, size);
-        }
-    } else {
-        EPID_FDISPATCH(in->dtype, run_median_generic, ctx, in, *out, size);
-    }
+    EPID_FDISPATCH(in->dtype, run_median, ctx, in, *out, size);
     return sync_and_check(ctx, rc, out);
 }
 

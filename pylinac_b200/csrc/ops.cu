@@ -1,5 +1,7 @@
 // Element-wise image operators with the reference's dtype semantics (core/array_utils.py:64-102,
-// core/image.py:785-815) and the public frame-statistics entry points.
+// core/image.py:785-815) and the public frame-statistics entry points.  Each operator computes in the batch's dtype;
+// array_utils chooses that dtype, the comparison type of threshold / binarize and the result dtype as numpy 2 does.
+// The per-frame min / max propagate NaN like numpy's a.min() / a.max(), wherever the NaN sits in the frame.
 #include <cmath>
 
 #include "filters.cuh"
@@ -15,6 +17,10 @@ template <> struct Wide<int16_t> { using type = int32_t; };
 // ---------------------------------------------------------------------------------------- per-frame min / max
 constexpr int MM_BLOCKS = 64, MM_THREADS = 256;
 
+// numpy's minimum / maximum: a NaN operand wins (v != v folds to false for integers)
+template <typename T> __device__ __forceinline__ T nan_min(T a, T v) { return (v < a || v != v) ? v : a; }
+template <typename T> __device__ __forceinline__ T nan_max(T a, T v) { return (v > a || v != v) ? v : a; }
+
 template <typename T>
 __global__ void __launch_bounds__(MM_THREADS) k_minmax_partial(const T* __restrict__ data, size_t per_frame, T* __restrict__ pmin, T* __restrict__ pmax) {
     const int fi = blockIdx.y;
@@ -22,8 +28,8 @@ __global__ void __launch_bounds__(MM_THREADS) k_minmax_partial(const T* __restri
     T mn = f[0], mx = f[0];
     for (size_t i = (size_t)blockIdx.x * MM_THREADS + threadIdx.x; i < per_frame; i += (size_t)MM_BLOCKS * MM_THREADS) {
         const T v = f[i];
-        mn = v < mn ? v : mn;
-        mx = v > mx ? v : mx;
+        mn = nan_min(mn, v);
+        mx = nan_max(mx, v);
     }
     __shared__ T smn[MM_THREADS], smx[MM_THREADS];
     smn[threadIdx.x] = mn;
@@ -31,9 +37,8 @@ __global__ void __launch_bounds__(MM_THREADS) k_minmax_partial(const T* __restri
     __syncthreads();
     for (int s = MM_THREADS / 2; s > 0; s >>= 1) {
         if (threadIdx.x < s) {
-            const T a = smn[threadIdx.x + s], b = smx[threadIdx.x + s];
-            if (a < smn[threadIdx.x]) smn[threadIdx.x] = a;
-            if (b > smx[threadIdx.x]) smx[threadIdx.x] = b;
+            smn[threadIdx.x] = nan_min(smn[threadIdx.x], smn[threadIdx.x + s]);
+            smx[threadIdx.x] = nan_max(smx[threadIdx.x], smx[threadIdx.x + s]);
         }
         __syncthreads();
     }
@@ -46,9 +51,8 @@ __global__ void k_minmax_final(const T* __restrict__ pmin, const T* __restrict__
     if (fi >= n) return;
     T a = pmin[fi * MM_BLOCKS], b = pmax[fi * MM_BLOCKS];
     for (int k = 1; k < MM_BLOCKS; k++) {
-        const T x = pmin[fi * MM_BLOCKS + k], y = pmax[fi * MM_BLOCKS + k];
-        a = x < a ? x : a;
-        b = y > b ? y : b;
+        a = nan_min(a, pmin[fi * MM_BLOCKS + k]);
+        b = nan_max(b, pmax[fi * MM_BLOCKS + k]);
     }
     mn[fi] = a;
     mx[fi] = b;
@@ -125,12 +129,6 @@ __global__ void k_binarize(const T* __restrict__ in, long long* __restrict__ out
         out[i] = ((double)in[i] >= t) ? 1 : 0;
 }
 
-template <typename T>
-__global__ void k_to_double(const T* __restrict__ in, double* __restrict__ out, int n) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) out[i] = (double)in[i];
-}
-
 #define EPID_DISPATCH(dt, FN, ...)                                                  \
     switch (dt) {                                                                   \
         case EPID_U8: rc = FN<uint8_t>(__VA_ARGS__); break;                         \
@@ -162,20 +160,13 @@ static int do_invert(epid_ctx* ctx, const epid_batch* in, epid_batch* out) {
 }
 
 template <typename T>
-static int do_ground(epid_ctx* ctx, const epid_batch* in, epid_batch* out, double value, double* mins) {
+static int do_ground(epid_ctx* ctx, const epid_batch* in, epid_batch* out, double value, void* mins) {
     T *mn, *mx;
     int rc = frame_minmax<T>(ctx, in, &mn, &mx);
     if (rc != EPID_OK) return rc;
     k_map_same<T, OP_GROUND><<<map_grid(in), 256, 0, ctx->stream>>>((const T*)in->dptr, (T*)out->dptr, (size_t)in->h * in->w, mn, mx, value);
     ctx->launches++;
-    if (mins) {
-        double* d = nullptr;
-        EPID_CUDA(cudaMallocAsync((void**)&d, sizeof(double) * in->n, ctx->stream));
-        k_to_double<T><<<(in->n + 127) / 128, 128, 0, ctx->stream>>>(mn, d, in->n);
-        ctx->launches++;
-        EPID_CUDA(cudaMemcpyAsync(mins, d, sizeof(double) * in->n, cudaMemcpyDeviceToHost, ctx->stream));
-        EPID_CUDA(cudaFreeAsync(d, ctx->stream));
-    }
+    if (mins) EPID_CUDA(cudaMemcpyAsync(mins, mn, sizeof(T) * in->n, cudaMemcpyDeviceToHost, ctx->stream));
     return EPID_OK;
 }
 
@@ -268,7 +259,7 @@ int32_t epid_bit_invert(epid_ctx* ctx, const epid_batch* in, epid_batch** out) {
     return finish(ctx, rc, out);
 }
 
-int32_t epid_ground(epid_ctx* ctx, const epid_batch* in, double value, epid_batch** out, double* mins) {
+int32_t epid_ground(epid_ctx* ctx, const epid_batch* in, double value, epid_batch** out, void* mins) {
     EPID_CHECK_IN(in);
     const bool is_float = in->dtype == EPID_F32 || in->dtype == EPID_F64;
     EPID_REQUIRE(is_float || value == floor(value), EPID_ERR_UNSUPPORTED, "ground(value) must be integral for integer images");
