@@ -890,6 +890,37 @@ int32_t epid_tu_stages(epid_ctx* ctx, const epid_batch* volumes, int32_t nz, int
                        struct epid_tu_result* results, double* mean, double* binned, double* filtered, double* cleaned, int32_t* edt2,
                        uint8_t* masks);
 
+/* CT phantom localization: pylinac.ct's Slice.phantom_roi (ct.py:381-433) with get_regions (ct.py:3315-3348) on the branch the
+ * cheese phantoms take (an ndarray, fill_holes, Otsu threshold, clip_in_localization), for every listed slice of an int16 or uint16
+ * series, each stage bit-identical to the numpy / scipy / skimage call it restates (DESIGN.md 4.19).  The row is a plain struct (not a
+ * typedef): its layout is checked by tests/test_cheese_host.py. */
+enum {
+    EPID_CT_OK = 0,
+    EPID_CT_NO_EDGES = 1,     /* max(scharr(HU)) < 0.1: "No edges were found ..." */
+    EPID_CT_NO_REGIONS = 2,   /* no region left after thresholding: "The number of ROIs detected ..." */
+    EPID_CT_WRONG_SIZE = 3    /* the closest region is more than 1.3x off catphan_size: "Unable to find ROI of expected size ..." */
+};
+struct epid_ct_slice { /* one per listed slice */
+    int32_t status;
+    int32_t n_regions;                 /* regions after the fill (0 when the edge check fails) */
+    int32_t label;                     /* raster index (row * w + col) of the chosen region's first pixel, -1 if none */
+    int32_t area;                      /* its area (= filled_area) */
+    double centroid_row;               /* coords.mean(axis=0) of its pixels (nan if none) */
+    double centroid_col;
+    double max_edge;                   /* max(scharr(HU)) */
+    double threshold;                  /* threshold_otsu of the smoothed edges */
+};
+/* slope / intercept: per slice of the whole series (index = slice); slices [nslices]: the slices to localize, results [nslices] on the
+ * host.  catphan_size: the expected area in px^2.  gauss_w [2 gauss_r + 1]: gaussian_filter1d's reversed weights for sigma 1 (mode
+ * 'nearest').  clip_in_localization 0 (a Slice passed to get_regions) returns EPID_ERR_UNSUPPORTED.  scharr, smoothed (float64),
+ * filled (uint8) and labels (int32: the union-find root of each pixel of the final mask as a chunk-wide index, -1 off it), each may
+ * be NULL: host planes [nslices][h][w] of the clipped Scharr edges, the smoothed edges, the mask after binary_fill_holes and its
+ * labels. */
+int32_t epid_ct_localize(epid_ctx* ctx, const epid_batch* volume, const double* slope, const double* intercept, const int32_t* slices,
+                         int32_t nslices, double catphan_size, int32_t clear_borders, int32_t clip_in_localization,
+                         const double* gauss_w, int32_t gauss_r, struct epid_ct_slice* results, double* scharr, double* smoothed,
+                         uint8_t* filled, int32_t* labels);
+
 /* ----------------------------------------------------------------------------------------- multi-GPU (NCCL)
  * The batch shards by frame index with no data-path collective; the only exchange is the final gather of the
  * fixed-size per-frame result structs (SURVEY.md 8e).  id: 128-byte ncclUniqueId created by rank 0. */

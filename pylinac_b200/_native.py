@@ -259,6 +259,12 @@ TU_RESULT_DTYPE = np.dtype([
     ("threshold", "<f8"), ("iu", "<f8", (3,)), ("du_max", "<f8", (6,)), ("center_sum", "<f8"), ("ring_sum", "<f8")], align=True)
 
 
+CT_OK, CT_NO_EDGES, CT_NO_REGIONS, CT_WRONG_SIZE = 0, 1, 2, 3
+
+CT_SLICE_DTYPE = np.dtype([("status", "<i4"), ("n_regions", "<i4"), ("label", "<i4"), ("area", "<i4"), ("centroid_row", "<f8"),
+                           ("centroid_col", "<f8"), ("max_edge", "<f8"), ("threshold", "<f8")], align=True)
+
+
 REGION_DTYPE = np.dtype([("threshold_index", "<i4"), ("label_root", "<i4"), ("bbox", "<i4", (4,)), ("area", "<f8"), ("area_filled", "<f8"),
                          ("perimeter", "<f8"), ("equivalent_diameter", "<f8"), ("centroid_y", "<f8"), ("centroid_x", "<f8"),
                          ("wcentroid_y", "<f8"), ("wcentroid_x", "<f8")], align=True)
@@ -340,6 +346,7 @@ _SIGNATURES = {
                            C.c_double, _P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)],
     "epid_tu_stages": [_P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_int32, C.c_double,
                        _P, _P, _P, _P, _P, _P, _P],
+    "epid_ct_localize": [_P, _P, _P, _P, _P, C.c_int32, C.c_double, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P],
     "epid_canny": [_P, _P, _P, C.c_int32, C.c_double, C.c_double, C.POINTER(_P)],
     "epid_hough_line": [_P, _P, C.c_int32, _P, C.POINTER(_P), C.POINTER(C.c_int32)],
     "epid_hough_candidates": [_P, _P, C.c_int32, C.c_int32, C.c_double, C.c_int32, _P, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
@@ -1074,6 +1081,40 @@ def tu_stages(ctx: Context, volumes, nz: int, first: int, count: int, bin_size: 
             float(threshold), _ptr(res), *(_ptr(a) for a in out.values())))
     out["results"] = res
     return out
+
+
+def ct_localize(ctx: Context, volume, slope, intercept, slices, catphan_size: float, clear_borders: bool,
+                clip_in_localization: bool = True, stages: bool = False):
+    """epid_ct_localize: the phantom localization of `slices` of an int16 / uint16 series (Batch [n, h, w] or ndarray) with per-slice
+    slope / intercept [n] -> CT_SLICE_DTYPE rows [len(slices)]; with `stages`, (rows, {"scharr", "smoothed" (float64), "filled" (bool),
+    "labels" (int32 skimage labels, 0 off the mask)} planes [len(slices), h, w])."""
+    sl = np.ascontiguousarray(slices, dtype=np.int32).reshape(-1)
+    w, lw = gaussian_kernel1d(1.0)
+    with batch_for(ctx, volume) as b:
+        (n, h, wd), _ = b.shape_dtype
+        sp = np.ascontiguousarray(np.broadcast_to(np.asarray(slope, np.float64), (n,)))
+        ic = np.ascontiguousarray(np.broadcast_to(np.asarray(intercept, np.float64), (n,)))
+        res = np.zeros(len(sl), CT_SLICE_DTYPE)
+        planes = None
+        if stages:
+            m = len(sl)
+            planes = {"scharr": np.empty((m, h, wd)), "smoothed": np.empty((m, h, wd)), "filled": np.empty((m, h, wd), np.uint8),
+                      "labels": np.empty((m, h, wd), np.int32)}
+        _unsupported_as_not_implemented(lib().epid_ct_localize(
+            ctx.handle, b.handle, _ptr(sp), _ptr(ic), _ptr(sl), len(sl), float(catphan_size), int(bool(clear_borders)),
+            int(bool(clip_in_localization)), _ptr(w), int(lw), _ptr(res), *(_ptr(a) for a in (planes or {}).values()),
+            *((None,) * (0 if planes else 4))))
+    if not stages:
+        return res
+    planes["filled"] = planes["filled"].view(bool)
+    lab = planes["labels"].reshape(len(sl), -1)
+    for k in range(len(sl)):      # union-find roots (chunk-wide indices) -> labels 1.. in raster order of each region's first pixel
+        fg = lab[k] >= 0
+        _, inv = np.unique(lab[k][fg], return_inverse=True)
+        out = np.zeros(lab.shape[1], np.int32)
+        out[fg] = inv + 1
+        lab[k] = out
+    return res, planes
 
 
 def divide(ctx: Context, num, den, sign_off=None) -> np.ndarray:

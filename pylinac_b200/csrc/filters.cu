@@ -8,8 +8,8 @@
 // k*k/2 is rank k/2 of the k-wide row window.  Tiles are sized per call, (32 + k - 1) x (8 + k - 1) keys for frames and
 // 256 + k - 1 keys for rows, up to the device's opt-in shared memory per block; a size no tile can hold is refused.
 //
-// correlate1d: scipy's symmetric / anti-symmetric summation order in fp64, mode='reflect', per-pass cast to the input
-// dtype.  The weights live in device memory allocated for the call on the context's stream, so any radius runs and two
+// correlate1d: scipy's symmetric / anti-symmetric summation order in fp64, mode='reflect' (or 'nearest' for the float64 passes
+// of ct.cu), per-pass cast to the input dtype.  The weights live in device memory allocated for the call on the context's stream, so any radius runs and two
 // contexts on one device never share them.
 #include <type_traits>
 
@@ -244,7 +244,8 @@ static int run_median(epid_ctx* ctx, const epid_batch* in, epid_batch* out, int 
 namespace epid {
 
 // One 1-D correlation pass along `axis` with scipy.ndimage.correlate1d's symmetric / anti-symmetric summation
-// order (ni_filters.c NI_Correlate1D), mode='reflect', fp64 accumulation, result cast to T.
+// order (ni_filters.c NI_Correlate1D), mode 'reflect' (nearest == 0) or 'nearest' (nearest == 1: a b | a b c d | c d), fp64
+// accumulation, result cast to T.
 //   sym > 0:  tmp = x[l]*w[r];  for ll = -r..-1: tmp += (x[l+ll] + x[l-ll]) * w[ll+r]
 //   sym < 0:  tmp = x[l]*w[r];  for ll = -r..-1: tmp += (x[l+ll] - x[l-ll]) * w[ll+r]
 //   sym == 0: tmp = sum_{ll=-r..r} x[l+ll] * w[ll+r]
@@ -260,7 +261,8 @@ template <> __device__ __forceinline__ int32_t cast_from_double<int32_t>(double 
 
 template <typename T>
 __global__ void __launch_bounds__(256)
-k_correlate1d(const T* __restrict__ in, T* __restrict__ out, const double* __restrict__ c_weights, int H, int W, int axis, int r, int sym) {
+k_correlate1d(const T* __restrict__ in, T* __restrict__ out, const double* __restrict__ c_weights, int H, int W, int axis, int r, int sym,
+              int nearest) {
     const int fi = blockIdx.z;
     const T* f = in + (size_t)fi * H * W;
     const int x = blockIdx.x * blockDim.x + threadIdx.x;
@@ -269,7 +271,7 @@ k_correlate1d(const T* __restrict__ in, T* __restrict__ out, const double* __res
     const int n = axis == 0 ? H : W;
     const int l = axis == 0 ? y : x;
     auto at = [&](int idx) -> double {
-        const int j = reflect_idx(idx, n);
+        const int j = nearest ? min(max(idx, 0), n - 1) : reflect_idx(idx, n);
         return (double)(axis == 0 ? f[(size_t)j * W + x] : f[(size_t)y * W + j]);
     };
     double tmp;
@@ -287,7 +289,7 @@ k_correlate1d(const T* __restrict__ in, T* __restrict__ out, const double* __res
 }
 
 template <typename T>
-static int run_correlate(epid_ctx* ctx, const void* in, void* out, int n, int H, int W, int axis, const double* w, int r) {
+static int run_correlate(epid_ctx* ctx, const void* in, void* out, int n, int H, int W, int axis, const double* w, int r, int nearest = 0) {
     // symmetry test as in scipy (ni_filters.c): |w[i] - w[2r-i]| <= DBL_EPSILON for all i -> symmetric
     int sym = 0;
     if (r > 0) {
@@ -304,7 +306,7 @@ static int run_correlate(epid_ctx* ctx, const void* in, void* out, int n, int H,
     cudaError_t e = cudaMemcpyAsync(d_w, w, sizeof(double) * (2 * r + 1), cudaMemcpyHostToDevice, ctx->stream);
     if (e == cudaSuccess) {
         dim3 grid((W + 255) / 256, H, n);
-        k_correlate1d<T><<<grid, 256, 0, ctx->stream>>>((const T*)in, (T*)out, d_w, H, W, axis, r, sym);
+        k_correlate1d<T><<<grid, 256, 0, ctx->stream>>>((const T*)in, (T*)out, d_w, H, W, axis, r, sym, nearest);
         ctx->launches++;
         e = cudaGetLastError();
     }
@@ -312,6 +314,10 @@ static int run_correlate(epid_ctx* ctx, const void* in, void* out, int n, int H,
     EPID_CUDA(e);
     EPID_CUDA(ef);
     return EPID_OK;
+}
+
+int correlate1d_f64(epid_ctx* ctx, const double* in, double* out, int n, int H, int W, int axis, const double* w, int r, int nearest) {
+    return run_correlate<double>(ctx, in, out, n, H, W, axis, w, r, nearest);
 }
 
 static int sync_and_check(epid_ctx* ctx, int rc, epid_batch** out) {

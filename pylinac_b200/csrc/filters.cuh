@@ -18,4 +18,8 @@ struct ValueMap {
 int launch_median_u16(epid_ctx* ctx, cudaStream_t stream, const FrameRef* d_src, const FrameRef* d_dst, const ValueMap* d_maps,
                       const int* d_select, int n, int H, int W, int k);
 
+// One scipy.ndimage.correlate1d pass over n compact float64 H x W frames on ctx->stream (filters.cu's k_correlate1d): weights w[2r + 1]
+// on the host, mode 'reflect' (nearest == 0) or 'nearest' (nearest == 1).  Asynchronous; returns a launch error.
+int correlate1d_f64(epid_ctx* ctx, const double* in, double* out, int n, int H, int W, int axis, const double* w, int r, int nearest);
+
 }  // namespace epid
