@@ -913,8 +913,8 @@ struct epid_ct_slice { /* one per listed slice */
 /* slope / intercept: per slice of the whole series (index = slice); slices [nslices]: the slices to localize, results [nslices] on the
  * host.  catphan_size: the expected area in px^2.  gauss_w [2 gauss_r + 1]: gaussian_filter1d's reversed weights for sigma 1 (mode
  * 'nearest').  clip_in_localization 0 (a Slice passed to get_regions) returns EPID_ERR_UNSUPPORTED.  scharr, smoothed (float64),
- * filled (uint8) and labels (int32: the union-find root of each pixel of the final mask as a chunk-wide index, -1 off it), each may
- * be NULL: host planes [nslices][h][w] of the clipped Scharr edges, the smoothed edges, the mask after binary_fill_holes and its
+ * filled (uint8) and labels (int32: the union-find root of each pixel of the final mask as an index within its slice, -1 off it), each
+ * may be NULL: host planes [nslices][h][w] of the clipped Scharr edges, the smoothed edges, the mask after binary_fill_holes and its
  * labels. */
 int32_t epid_ct_localize(epid_ctx* ctx, const epid_batch* volume, const double* slope, const double* intercept, const int32_t* slices,
                          int32_t nslices, double catphan_size, int32_t clear_borders, int32_t clip_in_localization,

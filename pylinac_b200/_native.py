@@ -1108,7 +1108,7 @@ def ct_localize(ctx: Context, volume, slope, intercept, slices, catphan_size: fl
         return res
     planes["filled"] = planes["filled"].view(bool)
     lab = planes["labels"].reshape(len(sl), -1)
-    for k in range(len(sl)):      # union-find roots (chunk-wide indices) -> labels 1.. in raster order of each region's first pixel
+    for k in range(len(sl)):      # union-find roots (indices within the slice) -> labels 1.. in raster order of each region's first pixel
         fg = lab[k] >= 0
         _, inv = np.unique(lab[k][fg], return_inverse=True)
         out = np.zeros(lab.shape[1], np.int32)

@@ -10,8 +10,8 @@
 //                 binary_fill_holes (background 4-connected to the outside stays); measure.label (8-connected); per region the
 //                 area and exact row / column sums
 //   k_ct_select   the region with the smallest |area - catphan_size| (first label on ties) and the 1.3x size check
-// Labels are union-find roots over the chunk's pixels (ccl.cuh): the smallest index of a component, which is skimage's raster label
-// order.  After the global fill every region's filled_area equals its area (no background is enclosed), so area stands for both.
+// Labels are union-find roots within each slice (ccl.cuh): the smallest index of a component, which is skimage's raster label order.
+// After the global fill every region's filled_area equals its area (no background is enclosed), so area stands for both.
 #include <cfloat>
 
 #include "ccl.cuh"
@@ -158,66 +158,58 @@ k_ct_otsu(const double* __restrict__ S, int HW, double* __restrict__ thres) {
     thres[blockIdx.x] = (edge[arg] + edge[arg + 1]) / 2.0;
 }
 
-__global__ void k_ct_binarize(const double* __restrict__ S, const double* __restrict__ thres, int HW, long long N, int* __restrict__ P) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < N) P[i] = S[i] > thres[i / HW] ? (int)i : -1;
+// The planes P and Q hold a chunk's slices one after the other, as union-find forests with slice-local parents: pixel i of the chunk
+// is pixel p = i % HW of its slice, whose planes start at i - p.  A chunk has at most CT_CHUNK_PIXELS pixels, so i is an int.
+
+__global__ void k_ct_binarize(const double* __restrict__ S, const double* __restrict__ thres, int HW, int N, int* __restrict__ P) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < N) P[i] = S[i] > thres[i / HW] ? i % HW : -1;
 }
 
-// union-find over the pixels with P >= 0: 8 neighbours (conn8) or 4, within each slice
-__global__ void k_ct_union(int H, int W, long long N, int conn8, int* __restrict__ P) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void k_ct_flatten(int HW, int N, int* __restrict__ P) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N || P[i] < 0) return;
-    const int p = (int)(i % ((long long)H * W)), y = p / W, x = p - y * W;
-    const int ii = (int)i;
-    const bool l = x > 0 && P[ii - 1] >= 0, u = y > 0 && P[ii - W] >= 0;
-    if (l) gl_union(P, ii, ii - 1);
-    if (u) gl_union(P, ii, ii - W);
-    if (conn8 && y > 0) {
-        if (!l && x > 0 && P[ii - W - 1] >= 0) gl_union(P, ii, ii - W - 1);
-        if (x + 1 < W && P[ii - W + 1] >= 0) gl_union(P, ii, ii - W + 1);
-    }
-}
-
-__global__ void k_ct_flatten(long long N, int* __restrict__ P) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < N && P[i] >= 0) P[i] = gl_find(P, (int)i);
+    const int p = i % HW;
+    P[i] = ccl_root(P + (i - p), p);
 }
 
 // flag[root] = 1 for every component of P with a pixel in the band of `ext` rows / columns along the slice's border
-__global__ void k_ct_mark_border(int H, int W, long long N, int ext, const int* __restrict__ P, int* __restrict__ flag) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void k_ct_mark_border(int H, int W, int N, int ext, const int* __restrict__ P, int* __restrict__ flag) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N || P[i] < 0) return;
-    const int p = (int)(i % ((long long)H * W)), y = p / W, x = p - y * W;
-    if (y < ext || y >= H - ext || x < ext || x >= W - ext) flag[P[i]] = 1;
+    const int p = i % (H * W), y = p / W, x = p - y * W;
+    if (y < ext || y >= H - ext || x < ext || x >= W - ext) flag[i - p + P[i]] = 1;
 }
 
-__global__ void k_ct_clear_flagged(long long N, int* __restrict__ P, const int* __restrict__ flag) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < N && P[i] >= 0 && flag[P[i]]) P[i] = -1;
+__global__ void k_ct_clear_flagged(int HW, int N, int* __restrict__ P, const int* __restrict__ flag) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < N && P[i] >= 0 && flag[i - i % HW + P[i]]) P[i] = -1;
 }
 
 // Q: the background (P < 0) as its own union-find forest
-__global__ void k_ct_background(long long N, const int* __restrict__ P, int* __restrict__ Q) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < N) Q[i] = P[i] < 0 ? (int)i : -1;
+__global__ void k_ct_background(int HW, int N, const int* __restrict__ P, int* __restrict__ Q) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < N) Q[i] = P[i] < 0 ? i % HW : -1;
 }
 
 // binary_fill_holes: a background pixel stays background when its 4-connected background component reaches the slice's edge
 // (flag[root] set by k_ct_mark_border with ext = 1).  P becomes the filled mask, ready to be labelled.
-__global__ void k_ct_fill(long long N, int* __restrict__ P, const int* __restrict__ Q, const int* __restrict__ flag, uint8_t* __restrict__ filled) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+__global__ void k_ct_fill(int HW, int N, int* __restrict__ P, const int* __restrict__ Q, const int* __restrict__ flag,
+                          uint8_t* __restrict__ filled) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N) return;
-    const bool fg = P[i] >= 0 || !flag[Q[i]];
-    P[i] = fg ? (int)i : -1;
+    const int p = i % HW;
+    const bool fg = P[i] >= 0 || !flag[i - p + Q[i]];
+    P[i] = fg ? p : -1;
     if (filled) filled[i] = fg ? 1 : 0;
 }
 
-__global__ void k_ct_region_sums(int H, int W, long long N, const int* __restrict__ P, unsigned int* __restrict__ area,
+__global__ void k_ct_region_sums(int H, int W, int N, const int* __restrict__ P, unsigned int* __restrict__ area,
                                  unsigned long long* __restrict__ rsum, unsigned long long* __restrict__ csum) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N || P[i] < 0) return;
-    const int p = (int)(i % ((long long)H * W)), y = p / W, x = p - y * W;
-    const int r = P[i];
+    const int p = i % (H * W), y = p / W, x = p - y * W;
+    const int r = i - p + P[i];
     atomicAdd(&area[r], 1u);
     if (y) atomicAdd(&rsum[r], (unsigned long long)y);
     if (x) atomicAdd(&csum[r], (unsigned long long)x);
@@ -244,7 +236,7 @@ k_ct_select(int HW, const int* __restrict__ P, const unsigned int* __restrict__ 
     const int base = s * HW;
     unsigned long long best = ~0ull, count = 0;
     for (int p = threadIdx.x; p < HW; p += blockDim.x) {
-        if (P[base + p] != base + p) continue;
+        if (P[base + p] != p) continue;
         count++;
         const double key = fabs((double)area[base + p] - catphan_size);
         best = min(best, (unsigned long long)__double_as_longlong(key));
@@ -253,7 +245,7 @@ k_ct_select(int HW, const int* __restrict__ P, const unsigned int* __restrict__ 
     // the first label among the best keys
     unsigned long long root = ~0ull;
     for (int p = threadIdx.x; p < HW; p += blockDim.x) {
-        if (P[base + p] != base + p) continue;
+        if (P[base + p] != p) continue;
         if ((unsigned long long)__double_as_longlong(fabs((double)area[base + p] - catphan_size)) == best) { root = p; break; }
     }
     root = block_min_u64(root, red);
@@ -287,7 +279,7 @@ k_ct_select(int HW, const int* __restrict__ P, const unsigned int* __restrict__ 
     }
 }
 
-inline unsigned blocks(long long N) { return (unsigned)((N + CT_THREADS - 1) / CT_THREADS); }
+inline unsigned blocks(int N) { return (unsigned)((N + CT_THREADS - 1) / CT_THREADS); }
 
 template <class T>
 int launch_scharr(epid_ctx* ctx, const SliceIn* d_in, int m, int H, int W, double* E, unsigned long long* emax) {
@@ -351,7 +343,8 @@ extern "C" int32_t epid_ct_localize(epid_ctx* ctx, const epid_batch* volume, con
     int rc = EPID_OK;
     for (int k0 = 0; k0 < nslices && rc == EPID_OK && e == cudaSuccess; k0 += chunk) {
         const int m = std::min(chunk, nslices - k0);
-        const long long N = HW * m;
+        const int N = (int)(HW * m);
+        const dim3 g_union(blocks((int)HW), m);      // one thread per pixel, slices in grid.y
         for (int j = 0; j < m; j++) {
             const int sl = slices[k0 + j];
             hin[j] = SliceIn{(const char*)volume->dptr + (size_t)sl * HW * esz, slope[sl], intercept[sl]};
@@ -367,22 +360,22 @@ extern "C" int32_t epid_ct_localize(epid_ctx* ctx, const epid_batch* volume, con
         k_ct_otsu<<<m, CT_SEL_THREADS, 0, ctx->stream>>>(S, (int)HW, d_thr);
         k_ct_binarize<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(S, d_thr, (int)HW, N, P);
         if (clear_borders) {
-            k_ct_union<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(H, W, N, 1, P);
-            k_ct_flatten<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(N, P);
+            k_ccl_union<<<g_union, CT_THREADS, 0, ctx->stream>>>(H, W, 1, P);
+            k_ct_flatten<<<blocks(N), CT_THREADS, 0, ctx->stream>>>((int)HW, N, P);
             e = cudaMemsetAsync(flag, 0, 4 * N, ctx->stream);
             if (e != cudaSuccess) break;
             k_ct_mark_border<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(H, W, N, ext, P, flag);
-            k_ct_clear_flagged<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(N, P, flag);
+            k_ct_clear_flagged<<<blocks(N), CT_THREADS, 0, ctx->stream>>>((int)HW, N, P, flag);
         }
-        k_ct_background<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(N, P, Q);
-        k_ct_union<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(H, W, N, 0, Q);
-        k_ct_flatten<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(N, Q);
+        k_ct_background<<<blocks(N), CT_THREADS, 0, ctx->stream>>>((int)HW, N, P, Q);
+        k_ccl_union<<<g_union, CT_THREADS, 0, ctx->stream>>>(H, W, 0, Q);
+        k_ct_flatten<<<blocks(N), CT_THREADS, 0, ctx->stream>>>((int)HW, N, Q);
         e = cudaMemsetAsync(flag, 0, 4 * N, ctx->stream);
         if (e != cudaSuccess) break;
         k_ct_mark_border<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(H, W, N, 1, Q, flag);
-        k_ct_fill<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(N, P, Q, flag, F);
-        k_ct_union<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(H, W, N, 1, P);
-        k_ct_flatten<<<blocks(N), CT_THREADS, 0, ctx->stream>>>(N, P);
+        k_ct_fill<<<blocks(N), CT_THREADS, 0, ctx->stream>>>((int)HW, N, P, Q, flag, F);
+        k_ccl_union<<<g_union, CT_THREADS, 0, ctx->stream>>>(H, W, 1, P);
+        k_ct_flatten<<<blocks(N), CT_THREADS, 0, ctx->stream>>>((int)HW, N, P);
         e = cudaMemsetAsync(A, 0, 4 * N, ctx->stream);
         if (e == cudaSuccess) e = cudaMemsetAsync(R, 0, 8 * N, ctx->stream);
         if (e == cudaSuccess) e = cudaMemsetAsync(Cs, 0, 8 * N, ctx->stream);

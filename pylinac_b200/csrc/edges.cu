@@ -6,7 +6,7 @@
 //                     mode='constant', truncate=4) as two correlate1d passes in scipy's symmetric summation order, divided by the
 //                     same filter of an all-ones mask (+ eps): skimage's bleed-over correction; k_canny_grad: ndimage.sobel along both
 //                     axes (mode 'reflect', scipy's anti-/symmetric summation order) + magnitude; k_canny_nms: bilinear non-maximum
-//                     suppression along the gradient; hysteresis = 8-connected components of the low mask (global union-find,
+//                     suppression along the gradient; hysteresis = 8-connected components of the low mask (k_ccl_union,
 //                     ccl.cuh) that contain a pixel >= the high threshold.
 //   epid_hough_line   every edge pixel votes for round(x cos t + y sin t) + offset at every angle (uint32 atomics on an L2-resident
 //                     accumulator): accumulator [2 * offset + 1][ntheta] as an int32 batch.
@@ -125,30 +125,13 @@ __global__ void k_hyst_init(const double* __restrict__ lowm, int* __restrict__ p
     }
 }
 
-__global__ void k_hyst_union(int H, int W, int* __restrict__ parent) {
-    const int f = blockIdx.y, HW = H * W;
-    int* par = parent + (size_t)f * HW;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x) {
-        if (par[i] < 0) continue;
-        const int y = i / W, x = i - y * W;
-        const bool l = x > 0 && par[i - 1] >= 0, u = y > 0 && par[i - W] >= 0;
-        if (l) gl_union(par, i, i - 1);
-        if (u) gl_union(par, i, i - W);
-        if (y > 0 && !u) {
-            if (!l && x > 0 && par[i - W - 1] >= 0) gl_union(par, i, i - W - 1);
-            if (x + 1 < W && par[i - W + 1] >= 0) gl_union(par, i, i - W + 1);
-        }
-    }
-}
-
 __global__ void k_hyst_mark(const double* __restrict__ lowm, int* __restrict__ parent, int* __restrict__ good, int HW, double high) {
     const int f = blockIdx.y;
     const size_t o = (size_t)f * HW;
     int* par = parent + o;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x) {
         if (par[i] < 0) continue;
-        int r = i;
-        while (par[r] != r) r = par[r];
+        const int r = ccl_root(par, i);
         if (r != i) par[i] = r;
         if (lowm[o + i] >= high) good[o + r] = 1;
     }
@@ -277,7 +260,7 @@ extern "C" int32_t epid_canny(epid_ctx* ctx, const epid_batch* in, const double*
     k_canny_nms<<<grid, ED_THREADS, 0, st>>>(d_i, d_j, d_mag, d_tmp, H, W, low_threshold);      // d_tmp = low_masked
     const dim3 g2(ctx->sm_count * 2, n);
     k_hyst_init<<<g2, 256, 0, st>>>(d_tmp, d_par, d_good, (int)per);
-    k_hyst_union<<<g2, 256, 0, st>>>(H, W, d_par);
+    k_ccl_union<<<g2, 256, 0, st>>>(H, W, 1, d_par);
     k_hyst_mark<<<g2, 256, 0, st>>>(d_tmp, d_par, d_good, (int)per, high_threshold);
     k_hyst_out<<<g2, 256, 0, st>>>(d_par, d_good, (uint8_t*)(*out)->dptr, (int)per);
     ctx->launches += 8;

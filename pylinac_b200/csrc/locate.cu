@@ -8,8 +8,8 @@
 //                    for (invert / stretch / normalise in the reference's operation order) is monotone in the raw pixel value, so
 //                    `sample > cutoff` is a threshold on the integer; found by bisection on that exact fp64 expression (once)
 //   k_gl_init        parent[i] = i for foreground pixels (-1 otherwise)
-//   k_gl_union       union-find merge with the left / upper neighbours (4-connectivity) or also the two upper diagonals (8), roots =
-//                    first pixel in raster order = skimage's label order
+//   k_ccl_union      ccl.cuh's union-find merge with the earlier neighbours (4- or 8-connectivity), roots = first pixel in raster
+//                    order = skimage's label order
 //   k_gl_flatten     parent[i] = root; root pixels reset their accumulators
 //   k_gl_props       area / bounding box per region, warp-aggregated atomics on root-indexed arrays
 //   k_gl_select      root pixels that survive clear_border and the cheap necessary conditions (area <= area_filled <= bbox area)
@@ -137,24 +137,6 @@ __global__ void k_gl_init(const uint16_t* __restrict__ frames, int HW, const GlF
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x) par[i] = live && gl_fg(F, k, img[i]) ? i : -1;
 }
 
-__global__ void k_gl_union(int H, int W, int conn8, int* __restrict__ parent) {
-    const int f = blockIdx.y, HW = H * W;
-    int* par = parent + (size_t)f * HW;
-    for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x) {
-        if (par[i] < 0) continue;
-        const int y = i / W, x = i - y * W;
-        const bool l = x > 0 && par[i - 1] >= 0, u = y > 0 && par[i - W] >= 0;
-        if (l) gl_union(par, i, i - 1);
-        if (u) gl_union(par, i, i - W);
-        if (conn8 && y > 0 && !u) {
-            // with the upper pixel set both upper diagonals are already joined through it; with the left pixel set the upper-left
-            // one is joined through that
-            if (!l && x > 0 && par[i - W - 1] >= 0) gl_union(par, i, i - W - 1);
-            if (x + 1 < W && par[i - W + 1] >= 0) gl_union(par, i, i - W + 1);
-        }
-    }
-}
-
 __global__ void k_gl_flatten(int HW, int W, int H, int* __restrict__ parent, unsigned int* __restrict__ area, unsigned int* __restrict__ bx0,
                              unsigned int* __restrict__ bx1, unsigned int* __restrict__ by0, unsigned int* __restrict__ by1) {
     const int f = blockIdx.y;
@@ -162,8 +144,7 @@ __global__ void k_gl_flatten(int HW, int W, int H, int* __restrict__ parent, uns
     int* par = parent + o;
     for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < HW; i += gridDim.x * blockDim.x) {
         if (par[i] < 0) continue;
-        int r = i;
-        while (par[r] != r) r = par[r];      // roots never change once the union kernel has finished
+        const int r = ccl_root(par, i);
         if (r == i) { area[o + i] = 0; bx0[o + i] = W; bx1[o + i] = 0; by0[o + i] = H; by1[o + i] = 0; }
         else par[i] = r;
     }
@@ -499,7 +480,7 @@ extern "C" int32_t epid_global_locate(epid_ctx* ctx, const epid_batch* frames, c
     const dim3 g(ctx->sm_count * 2, n);
     for (int k = 0; k < nthr_max; k++) {
         k_gl_init<<<g, 256, 0, ctx->stream>>>(fr, HW, d_gf, k, d_par, d_ncand);
-        k_gl_union<<<g, 256, 0, ctx->stream>>>(H, W, c.conn8, d_par);
+        k_ccl_union<<<g, 256, 0, ctx->stream>>>(H, W, c.conn8, d_par);
         k_gl_flatten<<<g, 256, 0, ctx->stream>>>(HW, W, H, d_par, d_area, d_x0, d_x1, d_y0, d_y1);
         k_gl_props<<<g, 256, 0, ctx->stream>>>(HW, W, d_par, d_area, d_x0, d_x1, d_y0, d_y1);
         k_gl_select<<<g, 256, 0, ctx->stream>>>(c, d_par, d_area, d_x0, d_x1, d_y0, d_y1, d_cand, d_ncand);

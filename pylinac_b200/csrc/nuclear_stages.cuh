@@ -69,8 +69,7 @@ __device__ __forceinline__ void label_areas(int* P, int* A, int hb, int wb) {
     for (int p = tid; p < N; p += nt) {
         if (P[p] < 0) continue;
         const int i = p / wb, j = p - i * wb;
-        if (j > 0 && P[p - 1] >= 0) gl_union(P, p, p - 1);
-        if (i > 0 && P[p - wb] >= 0) gl_union(P, p, p - wb);
+        ccl_join(P, p, j, i, wb, false);
     }
     __syncthreads();
     for (int p = tid; p < N; p += nt) {

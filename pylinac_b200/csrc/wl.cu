@@ -368,26 +368,6 @@ struct WlComp {
     int root[WL_MAXC];
 };
 
-__device__ __forceinline__ int wl_find(volatile int* parent, int i) {
-    while (true) {
-        const int p = parent[i];
-        if (p == i) return i;
-        i = p;
-    }
-}
-
-__device__ __forceinline__ void wl_union(int* parent, int a, int b) {
-    while (true) {
-        a = wl_find(parent, a);
-        b = wl_find(parent, b);
-        if (a == b) return;
-        if (a < b) { const int t = a; a = b; b = t; }      // a > b: hook the larger root under the smaller one
-        const int old = atomicMin(&parent[a], b);
-        if (old == a) return;
-        a = old;
-    }
-}
-
 __global__ void __launch_bounds__(WL_THREADS)
 k_wl_bb(const WlConst* __restrict__ cc, const uint16_t* __restrict__ base, const WlFrame* __restrict__ wf, double* __restrict__ samples,
         unsigned short* __restrict__ cid_all, WlComp* __restrict__ comp_all, epid_wl_result* __restrict__ res,

@@ -88,7 +88,7 @@ def main():
         kern = {}
         for ev in prof.key_averages():
             if ev.device_type.name == "CUDA" and (ev.key.startswith("_ZN") or "k_" in ev.key):
-                name = next((k for k in ("k_ct_scharr", "k_correlate1d", "k_ct_otsu", "k_ct_binarize", "k_ct_union", "k_ct_flatten",
+                name = next((k for k in ("k_ct_scharr", "k_correlate1d", "k_ct_otsu", "k_ct_binarize", "k_ccl_union", "k_ct_flatten",
                                          "k_ct_mark_border", "k_ct_clear_flagged", "k_ct_background", "k_ct_fill", "k_ct_region_sums",
                                          "k_ct_select") if k in ev.key), ev.key[:40])
                 kern[name] = kern.get(name, 0.0) + ev.device_time_total / 1000.0
