@@ -890,10 +890,12 @@ int32_t epid_tu_stages(epid_ctx* ctx, const epid_batch* volumes, int32_t nz, int
                        struct epid_tu_result* results, double* mean, double* binned, double* filtered, double* cleaned, int32_t* edt2,
                        uint8_t* masks);
 
-/* CT phantom localization: pylinac.ct's Slice.phantom_roi (ct.py:381-433) with get_regions (ct.py:3315-3348) on the branch the
- * cheese phantoms take (an ndarray, fill_holes, Otsu threshold, clip_in_localization), for every listed slice of an int16 or uint16
- * series, each stage bit-identical to the numpy / scipy / skimage call it restates (DESIGN.md 4.19).  The row is a plain struct (not a
- * typedef): its layout is checked by tests/test_cheese_host.py. */
+/* CT phantom localization: pylinac.ct's Slice.phantom_roi (ct.py:381-433) with get_regions (ct.py:3315-3348, fill_holes, Otsu
+ * threshold), for every listed slice of an int16 or uint16 series, each stage bit-identical to the numpy / scipy / skimage call it
+ * restates (DESIGN.md 4.19, 4.20).  Both branches of get_regions: the ndarray branch (clip_in_localization, the cheese phantoms) and
+ * the Slice branch (CatPhanBase's default, ct.py:403-406 and 3326-3340: Otsu over skimage.draw.disk(image centre, 110 mm) times 0.8,
+ * no clipping).  The rows are plain structs (not typedefs): their layouts are checked by tests/test_cheese_host.py and
+ * tests/test_acr_host.py. */
 enum {
     EPID_CT_OK = 0,
     EPID_CT_NO_EDGES = 1,     /* max(scharr(HU)) < 0.1: "No edges were found ..." */
@@ -908,18 +910,40 @@ struct epid_ct_slice { /* one per listed slice */
     double centroid_row;               /* coords.mean(axis=0) of its pixels (nan if none) */
     double centroid_col;
     double max_edge;                   /* max(scharr(HU)) */
-    double threshold;                  /* threshold_otsu of the smoothed edges */
+    double threshold;                  /* threshold_otsu of the smoothed edges (times 0.8 on the Slice branch) */
 };
-/* slope / intercept: per slice of the whole series (index = slice); slices [nslices]: the slices to localize, results [nslices] on the
- * host.  catphan_size: the expected area in px^2.  gauss_w [2 gauss_r + 1]: gaussian_filter1d's reversed weights for sigma 1 (mode
- * 'nearest').  clip_in_localization 0 (a Slice passed to get_regions) returns EPID_ERR_UNSUPPORTED.  scharr, smoothed (float64),
- * filled (uint8) and labels (int32: the union-find root of each pixel of the final mask as an index within its slice, -1 off it), each
- * may be NULL: host planes [nslices][h][w] of the clipped Scharr edges, the smoothed edges, the mask after binary_fill_holes and its
- * labels. */
+/* ct.py:381-433 Slice.phantom_roi for every listed slice.  slope / intercept: per slice of the whole series (index = slice); slices
+ * [nslices]: the slices to localize, results [nslices] on the host.  catphan_size: the expected area in px^2.  gauss_w
+ * [2 gauss_r + 1]: gaussian_filter1d's reversed weights for sigma 1 (mode 'nearest').  otsu_disk_radius > 0 (at least 1 pixel)
+ * selects the Slice branch, which requires clip_in_localization 0; otsu_disk_radius <= 0 the ndarray branch, which requires
+ * clip_in_localization 1.  clip_in_localization 0 without a disk returns EPID_ERR_UNSUPPORTED, a disk with clipping EPID_ERR_INVALID.
+ * scharr, smoothed (float64), filled (uint8) and labels (int32: the union-find root of each pixel of the final mask as an index within
+ * its slice, -1 off it), each may be NULL: host planes [nslices][h][w] of the Scharr edges the Gaussian smooths (of the clipped HU on
+ * the ndarray branch, of the HU on the Slice branch), the smoothed edges, the mask after binary_fill_holes and its labels. */
 int32_t epid_ct_localize(epid_ctx* ctx, const epid_batch* volume, const double* slope, const double* intercept, const int32_t* slices,
                          int32_t nslices, double catphan_size, int32_t clear_borders, int32_t clip_in_localization,
-                         const double* gauss_w, int32_t gauss_r, struct epid_ct_slice* results, double* scharr, double* smoothed,
-                         uint8_t* filled, int32_t* labels);
+                         double otsu_disk_radius, const double* gauss_w, int32_t gauss_r, struct epid_ct_slice* results,
+                         double* scharr, double* smoothed, uint8_t* filled, int32_t* labels);
+
+struct epid_ct_region { /* one per region of get_regions(slice), in skimage's label order */
+    int32_t label;                     /* skimage's label: 1 + the region's rank in raster order of first pixels */
+    int32_t first;                     /* raster index (row * w + col) of the region's first pixel */
+    int32_t area;
+    int32_t filled_area;               /* binary_fill_holes of the region's own bbox crop (4-connected background) */
+    int32_t bbox[4];                   /* min_row, min_col, max_row + 1, max_col + 1, as skimage's bbox */
+    uint64_t sum_r;                    /* exact sums of the pixels' rows and columns: centroid = sum / area */
+    uint64_t sum_c;
+    uint64_t m_rr;                     /* exact second moments about the bbox corner: sum (r - min_row)^2, sum (c - min_col)^2, */
+    uint64_t m_cc;                     /* sum (r - min_row) (c - min_col) */
+    uint64_t m_rc;
+};
+/* ct.py:3315-3348 get_regions(slice) with its defaults, as CatPhanBase.find_phantom_roll (ct.py:2541) calls it, for one slice: the
+ * Slice branch's Scharr, Gaussian and disk Otsu times 0.8 (otsu_disk_radius > 0, at least 1 pixel), clear_border, no hole filling,
+ * 8-connected labels.  regions [capacity] on the host gets the first min(count, capacity) rows; *count the number of regions,
+ * *threshold the slice's threshold and *max_edge max(scharr(HU)).  The other arguments are epid_ct_localize's. */
+int32_t epid_ct_regions(epid_ctx* ctx, const epid_batch* volume, const double* slope, const double* intercept, int32_t slice,
+                        double otsu_disk_radius, const double* gauss_w, int32_t gauss_r, struct epid_ct_region* regions,
+                        int32_t capacity, int32_t* count, double* threshold, double* max_edge);
 
 /* ----------------------------------------------------------------------------------------- multi-GPU (NCCL)
  * The batch shards by frame index with no data-path collective; the only exchange is the final gather of the

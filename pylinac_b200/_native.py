@@ -264,6 +264,9 @@ CT_OK, CT_NO_EDGES, CT_NO_REGIONS, CT_WRONG_SIZE = 0, 1, 2, 3
 CT_SLICE_DTYPE = np.dtype([("status", "<i4"), ("n_regions", "<i4"), ("label", "<i4"), ("area", "<i4"), ("centroid_row", "<f8"),
                            ("centroid_col", "<f8"), ("max_edge", "<f8"), ("threshold", "<f8")], align=True)
 
+CT_REGION_DTYPE = np.dtype([("label", "<i4"), ("first", "<i4"), ("area", "<i4"), ("filled_area", "<i4"), ("bbox", "<i4", (4,)),
+                            ("sum_r", "<u8"), ("sum_c", "<u8"), ("m_rr", "<u8"), ("m_cc", "<u8"), ("m_rc", "<u8")], align=True)
+
 
 REGION_DTYPE = np.dtype([("threshold_index", "<i4"), ("label_root", "<i4"), ("bbox", "<i4", (4,)), ("area", "<f8"), ("area_filled", "<f8"),
                          ("perimeter", "<f8"), ("equivalent_diameter", "<f8"), ("centroid_y", "<f8"), ("centroid_x", "<f8"),
@@ -346,7 +349,9 @@ _SIGNATURES = {
                            C.c_double, _P, C.POINTER(_P), C.POINTER(_P), C.POINTER(_P)],
     "epid_tu_stages": [_P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_double, C.c_double, C.c_double, C.c_int32, C.c_double,
                        _P, _P, _P, _P, _P, _P, _P],
-    "epid_ct_localize": [_P, _P, _P, _P, _P, C.c_int32, C.c_double, C.c_int32, C.c_int32, _P, C.c_int32, _P, _P, _P, _P, _P],
+    "epid_ct_localize": [_P, _P, _P, _P, _P, C.c_int32, C.c_double, C.c_int32, C.c_int32, C.c_double, _P, C.c_int32, _P, _P, _P, _P,
+                         _P],
+    "epid_ct_regions": [_P, _P, _P, _P, C.c_int32, C.c_double, _P, C.c_int32, _P, C.c_int32, _P, _P, _P],
     "epid_canny": [_P, _P, _P, C.c_int32, C.c_double, C.c_double, C.POINTER(_P)],
     "epid_hough_line": [_P, _P, C.c_int32, _P, C.POINTER(_P), C.POINTER(C.c_int32)],
     "epid_hough_candidates": [_P, _P, C.c_int32, C.c_int32, C.c_double, C.c_int32, _P, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
@@ -1084,10 +1089,11 @@ def tu_stages(ctx: Context, volumes, nz: int, first: int, count: int, bin_size: 
 
 
 def ct_localize(ctx: Context, volume, slope, intercept, slices, catphan_size: float, clear_borders: bool,
-                clip_in_localization: bool = True, stages: bool = False):
+                clip_in_localization: bool = True, stages: bool = False, otsu_disk_radius: float = 0.0):
     """epid_ct_localize: the phantom localization of `slices` of an int16 / uint16 series (Batch [n, h, w] or ndarray) with per-slice
     slope / intercept [n] -> CT_SLICE_DTYPE rows [len(slices)]; with `stages`, (rows, {"scharr", "smoothed" (float64), "filled" (bool),
-    "labels" (int32 skimage labels, 0 off the mask)} planes [len(slices), h, w])."""
+    "labels" (int32 skimage labels, 0 off the mask)} planes [len(slices), h, w]).  otsu_disk_radius > 0 (pixels) with
+    clip_in_localization False is get_regions' Slice branch; 0 with clip_in_localization True its ndarray branch."""
     sl = np.ascontiguousarray(slices, dtype=np.int32).reshape(-1)
     w, lw = gaussian_kernel1d(1.0)
     with batch_for(ctx, volume) as b:
@@ -1102,7 +1108,7 @@ def ct_localize(ctx: Context, volume, slope, intercept, slices, catphan_size: fl
                       "labels": np.empty((m, h, wd), np.int32)}
         _unsupported_as_not_implemented(lib().epid_ct_localize(
             ctx.handle, b.handle, _ptr(sp), _ptr(ic), _ptr(sl), len(sl), float(catphan_size), int(bool(clear_borders)),
-            int(bool(clip_in_localization)), _ptr(w), int(lw), _ptr(res), *(_ptr(a) for a in (planes or {}).values()),
+            int(bool(clip_in_localization)), float(otsu_disk_radius), _ptr(w), int(lw), _ptr(res), *(_ptr(a) for a in (planes or {}).values()),
             *((None,) * (0 if planes else 4))))
     if not stages:
         return res
@@ -1115,6 +1121,27 @@ def ct_localize(ctx: Context, volume, slope, intercept, slices, catphan_size: fl
         out[fg] = inv + 1
         lab[k] = out
     return res, planes
+
+
+def ct_regions(ctx: Context, volume, slope, intercept, slice_num: int, otsu_disk_radius: float, capacity: int = 64):
+    """epid_ct_regions: get_regions(slice) of slice `slice_num` of an int16 / uint16 series (Batch [n, h, w] or ndarray) with per-slice
+    slope / intercept [n] -> (CT_REGION_DTYPE rows in label order, threshold, max_edge).  A table longer than `capacity` is read again
+    with room for all of it."""
+    w, lw = gaussian_kernel1d(1.0)
+    with batch_for(ctx, volume) as b:
+        (n, _, _), _ = b.shape_dtype
+        sp = np.ascontiguousarray(np.broadcast_to(np.asarray(slope, np.float64), (n,)))
+        ic = np.ascontiguousarray(np.broadcast_to(np.asarray(intercept, np.float64), (n,)))
+        cap = max(int(capacity), 1)
+        while True:
+            rows = np.zeros(cap, CT_REGION_DTYPE)
+            count, thres, max_edge = C.c_int32(), C.c_double(), C.c_double()
+            _unsupported_as_not_implemented(lib().epid_ct_regions(
+                ctx.handle, b.handle, _ptr(sp), _ptr(ic), int(slice_num), float(otsu_disk_radius), _ptr(w), int(lw), _ptr(rows), cap,
+                C.byref(count), C.byref(thres), C.byref(max_edge)))
+            if count.value <= cap:
+                return rows[:count.value], thres.value, max_edge.value
+            cap = count.value
 
 
 def divide(ctx: Context, num, den, sign_off=None) -> np.ndarray:

@@ -145,6 +145,10 @@ class CheesePhantomBase(CatPhanBase, ResultsDataMixin[CheeseResult]):
         self.module = self.module_class(self, clear_borders=self.clear_borders)
         self.roi_config = roi_config
 
+    def _ensure_physical_scan_extent(self) -> bool:
+        """cheese.py:303-305: a cheese phantom has one module, always in the scan."""
+        return True
+
     def _roi_angles(self) -> list[float]:
         return [wrap360(s["angle"]) for s in self.module_class.roi_settings.values()]
 

@@ -91,7 +91,8 @@ def capture_warnings(cls):
         if parent is object:
             continue
         for name, attr in parent.__dict__.items():
-            if name.startswith("_") or name in own:
+            # the live dict: the first class of the MRO that defines a method wins, as in attribute lookup
+            if name.startswith("_") or name in cls.__dict__:
                 continue
             if is_func(attr):
                 setattr(cls, name, capture_warnings_method_wrapper(attr))

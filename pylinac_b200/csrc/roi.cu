@@ -213,20 +213,6 @@ template <> struct DiskTraits<double> {
 
 struct DiskOut { double count, mean, std, mn, mx, median; };   // count < 0: a member pixel lies beyond the frame (numpy's IndexError)
 
-// skimage.draw.disk's bounding box of one disk: rows r0 .. r0 + bh - 1, columns c0 .. c0 + bw - 1 (bh, bw >= 0)
-struct DiskBox { long long r0, c0, bh, bw; };
-__host__ __device__ inline DiskBox disk_box(double cy, double cx, double R) {
-    R = fabs(R);                                     // skimage's rotated radius |r cos 0| + r sin 0
-    DiskBox b;
-    b.r0 = (long long)ceil(cy - R);
-    b.c0 = (long long)ceil(cx - R);
-    b.bh = (long long)floor(cy + R) - b.r0 + 1;
-    b.bw = (long long)floor(cx + R) - b.c0 + 1;
-    if (b.bh < 0) b.bh = 0;
-    if (b.bw < 0) b.bw = 0;
-    return b;
-}
-
 // member j of row i of a disk's row table, negative indices wrapped as numpy's fancy indexing does
 template <typename T> struct DiskPixel {
     const T* f;

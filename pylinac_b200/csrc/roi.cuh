@@ -1,8 +1,25 @@
-// Point-in-quadrilateral rule shared by the ROI kernels (roi.cu, vmat.cu): the pixel selection of RectangleROI.pixels_flat
-// (core/roi.py:641-660 -> skimage.draw.polygon): integer pixel coordinates inside the corner polygon or ON its boundary.
+// Pixel-selection rules shared by the ROI kernels (roi.cu, vmat.cu) and the CT localization (ct.cu): skimage.draw.disk's bounding box,
+// and the point-in-quadrilateral rule of RectangleROI.pixels_flat (core/roi.py:641-660 -> skimage.draw.polygon): integer pixel
+// coordinates inside the corner polygon or ON its boundary.
 #pragma once
 
+#include <cmath>
+
 namespace epid {
+
+// skimage.draw.disk's bounding box of one disk: rows r0 .. r0 + bh - 1, columns c0 .. c0 + bw - 1 (bh, bw >= 0)
+struct DiskBox { long long r0, c0, bh, bw; };
+__host__ __device__ inline DiskBox disk_box(double cy, double cx, double R) {
+    R = fabs(R);                                     // skimage's rotated radius |r cos 0| + r sin 0
+    DiskBox b;
+    b.r0 = (long long)ceil(cy - R);
+    b.c0 = (long long)ceil(cx - R);
+    b.bh = (long long)floor(cy + R) - b.r0 + 1;
+    b.bw = (long long)floor(cx + R) - b.c0 + 1;
+    if (b.bh < 0) b.bh = 0;
+    if (b.bw < 0) b.bw = 0;
+    return b;
+}
 
 // 0 outside, non-zero inside or on the boundary (crossing number with explicit edge / vertex tests, the structure of skimage's
 // _geometry.point_in_polygon)
